@@ -230,6 +230,34 @@ int vp_device_zero(void* device_ptr, size_t nbytes, void* stream);
  * (infer_utils/speaker_diarization.py:254-257). */
 int vp_cosine_scores(vp_handle* h, const float* a, int32_t n, const float* b, int32_t m, int32_t D, float* scores, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Spectral stage of the diarization clustering: SpectralCluster.__call__ (infer_utils/speaker_diarization.py:235-250)
+ * up to its eigenvectors, in fp64 after the affinity.  The tridiagonal eigenproblem in between (2n numbers down, [n, k]
+ * up) is the caller's: mvector/engine.py::spectral_embedding solves it with LAPACK stebz/stein.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* device scratch bytes that vp_spectral_laplacian and vp_sym_tridiag need for an n-point problem (n^2 floats at most) */
+size_t vp_spectral_scratch_bytes(const vp_handle* h, int32_t n);
+/* emb [n, D] float32 -> L [n, n] float64 (row-major, both triangles), the unnormalised Laplacian of the pruned affinity:
+ *   S0 = cosine(emb, emb)                       (get_sim_mat, :253-257; the vp_cosine_scores kernel)
+ *   P  = S0 with the n_drop smallest entries of every row set to 0   (p_pruning, :260-274); ties at the cut go by column
+ *        index, lower indices first (numpy's stable argsort; the reference's default quicksort leaves that order open)
+ *   S  = 0.5 (P + P') in fp64, zero diagonal; d_i = sum_j |S_ij|; L = diag(d) - S   (:246, get_laplacian :277-283)
+ * n_drop = len(range(n)[:int((1 - pval) * n)]) as Python evaluates p_pruning's expression, in [0, n).  n <= 58 000. */
+int vp_spectral_laplacian(vp_handle* h, const float* emb, int32_t n, int32_t D, int32_t n_drop, double* L, void* scratch,
+                          void* stream);
+/* In-place Householder reduction of a symmetric A [n, n] (float64, full storage) to T = Q' A Q = tridiag(d, e), LAPACK
+ * dsytd2 with UPLO = 'L': H_k = I - tau[k] v v', v = (0.., 1, A[k+2:, k]), beta = -sign(alpha) ||x||.  On return the
+ * diagonal and first subdiagonal of A hold d and e, the strictly lower part below it the reflectors; the upper triangle
+ * is scratch.  d [n], e [n-1], tau [n-1] (tau[n-2] = 0) are device float64.  Replaces the dense scipy.linalg.eigh of
+ * get_spec_embs (:285-295) up to the tridiagonal eigenproblem. */
+int vp_sym_tridiag(vp_handle* h, double* A, int32_t n, double* d, double* e, double* tau, void* scratch, void* stream);
+/* Z [n, k] (float64, row-major, device) <- Q Z with the reflectors vp_sym_tridiag left in A and tau: eigenvectors of T
+ * become eigenvectors of the original matrix.  1 <= k <= min(n, 16) (get_spec_embs keeps <= max_num_spks = 15 columns). */
+int vp_sym_tridiag_apply_q(vp_handle* h, const double* A, const double* tau, int32_t n, double* Z, int32_t k,
+                           void* stream);
+/* kernel launches of one vp_spectral_laplacian + vp_sym_tridiag + vp_sym_tridiag_apply_q at size n */
+int32_t vp_spectral_launches(int32_t n);
+
 /* Staging half of predict_batch (predict.py:244-255) as ONE native call: worker threads gather slices of slice_rows
  * utterances into the zero-padded PINNED matrix staging[n, lmax]; the calling thread -- one of the n_threads gatherers --
  * issues cudaMemcpyAsync(staging slice -> device_dst slice) on copy_stream, in slice order, as soon as a slice is

@@ -763,6 +763,44 @@ int vp_cosine_scores(vp_handle* h, const float* a, int32_t n, const float* b, in
   return VP_OK;
 }
 
+size_t vp_spectral_scratch_bytes(const vp_handle* h, int32_t n) {
+  (void)h;
+  return n < 1 ? 0 : spectral_scratch_bytes(n);
+}
+
+int vp_spectral_laplacian(vp_handle* h, const float* emb, int32_t n, int32_t D, int32_t n_drop, double* L, void* scratch,
+                          void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (!emb || !L || !scratch || n < 1 || D < 1) return fail(h, VP_ERR_INVALID, "null/empty argument");
+  if (n_drop < 0 || n_drop >= n) return fail(h, VP_ERR_INVALID, "n_drop %d outside [0, n = %d)", n_drop, n);
+  if ((size_t)n * sizeof(unsigned) > 227 * 1024)
+    return fail(h, VP_ERR_UNSUPPORTED, "n = %d: a row of the affinity no longer fits in shared memory", n);
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_spectral_laplacian(emb, n, D, n_drop, L, scratch, (cudaStream_t)stream));
+  return VP_OK;
+}
+
+int vp_sym_tridiag(vp_handle* h, double* A, int32_t n, double* d, double* e, double* tau, void* scratch, void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (!A || !d || !scratch || n < 1 || (n > 1 && (!e || !tau))) return fail(h, VP_ERR_INVALID, "null/empty argument");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_sym_tridiag(A, n, d, e, tau, scratch, (cudaStream_t)stream));
+  return VP_OK;
+}
+
+int vp_sym_tridiag_apply_q(vp_handle* h, const double* A, const double* tau, int32_t n, double* Z, int32_t k, void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (!A || !Z || n < 1 || (n > 1 && !tau)) return fail(h, VP_ERR_INVALID, "null/empty argument");
+  if (k < 1 || k > n || k > 16) return fail(h, VP_ERR_INVALID, "k = %d outside [1, min(n, 16)] (n = %d)", k, n);
+  if ((n + 7) / 8 > apply_q_max_rows(k))
+    return fail(h, VP_ERR_UNSUPPORTED, "n = %d, k = %d: the [n, k] block does not fit in the shared memory of 8 CTAs", n, k);
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_sym_tridiag_apply_q(A, tau, n, Z, k, (cudaStream_t)stream));
+  return VP_OK;
+}
+
+int32_t vp_spectral_launches(int32_t n) { return n < 1 ? 0 : spectral_launches_laplacian() + spectral_launches_tridiag(n) + 1; }
+
 int vp_program_peek(vp_program* p, int64_t off, size_t nbytes, void* dst, void* stream) {
   if (!p || !dst) return VP_ERR_INVALID;
   if (off < 0 || (size_t)off + nbytes > p->ws_bytes) return fail(p->h, VP_ERR_INVALID, "peek out of range");

@@ -51,6 +51,15 @@ struct PoolParams {
 cudaError_t launch_pool2d(const PoolParams& p, cudaStream_t stream);
 cudaError_t launch_cosine_scores(const float* a, const float* b, float* out, int n, int m, int D, cudaStream_t stream);
 
+// spectral stage of the diarization clustering (spectral.cu)
+size_t spectral_scratch_bytes(int n);
+int spectral_launches_laplacian();
+int spectral_launches_tridiag(int n);
+int apply_q_max_rows(int kz);
+cudaError_t launch_spectral_laplacian(const float* emb, int n, int D, int n_drop, double* L, void* scratch, cudaStream_t stream);
+cudaError_t launch_sym_tridiag(double* A, int n, double* d, double* e, double* tau, void* scratch, cudaStream_t stream);
+cudaError_t launch_sym_tridiag_apply_q(const double* A, const double* tau, int n, double* Z, int kz, cudaStream_t stream);
+
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);

@@ -91,6 +91,11 @@ def lib():
         'vp_workspace_bytes': (sz, [vp]),
         'vp_device_zero': (C.c_int, [C.c_void_p, sz, vp]),
         'vp_cosine_scores': (C.c_int, [vp, f32p, i32, f32p, i32, i32, f32p, vp]),
+        'vp_spectral_scratch_bytes': (sz, [vp, i32]),
+        'vp_spectral_laplacian': (C.c_int, [vp, f32p, i32, i32, i32, C.c_void_p, C.c_void_p, vp]),
+        'vp_sym_tridiag': (C.c_int, [vp, C.c_void_p, i32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, vp]),
+        'vp_sym_tridiag_apply_q': (C.c_int, [vp, C.c_void_p, C.c_void_p, i32, C.c_void_p, i32, vp]),
+        'vp_spectral_launches': (i32, [i32]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = header/library mismatch
@@ -109,4 +114,6 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_feature_dim',
            'vp_weights_load', 'vp_program_create', 'vp_program_destroy', 'vp_embed', 'vp_embed_wave',
            'vp_program_launches', 'vp_program_peek', 'vp_embed_profiled', 'vp_program_op_info', 'vp_host_gather_pad',
-           'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_cosine_scores', 'vp_device_zero']
+           'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_cosine_scores', 'vp_device_zero',
+           'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
+           'vp_spectral_launches']

@@ -61,6 +61,70 @@ class Engine:
                                                  tb.shape[0], ta.shape[1], C.c_void_p(out.data_ptr()), self.stream_ptr()))
         return out
 
+    # ---- spectral stage of the diarization clustering (csrc/spectral.cu) ----
+    def spectral_scratch(self, n):
+        """Device scratch for spectral_laplacian / sym_tridiag at size n (uint8 tensor)."""
+        return torch.empty(int(L.lib().vp_spectral_scratch_bytes(self._h, n)), dtype=torch.uint8, device=self.device)
+
+    def spectral_laplacian(self, X, n_drop, scratch=None):
+        """[n, D] embeddings -> device float64 [n, n] unnormalised Laplacian of the pruned cosine affinity
+        (vp_spectral_laplacian)."""
+        tx = torch.as_tensor(X, dtype=torch.float32).to(self.device).contiguous()
+        n, D = tx.shape
+        scratch = self.spectral_scratch(n) if scratch is None else scratch
+        Lm = torch.empty(n, n, dtype=torch.float64, device=self.device)
+        _check(self._h, L.lib().vp_spectral_laplacian(self._h, C.c_void_p(tx.data_ptr()), n, D, int(n_drop),
+                                                      C.c_void_p(Lm.data_ptr()), C.c_void_p(scratch.data_ptr()),
+                                                      self.stream_ptr()))
+        return Lm
+
+    def sym_tridiag(self, A, scratch=None):
+        """In place on the device float64 symmetric A [n, n]: Householder reduction to tridiag(d, e); -> device
+        (d [n], e [n-1], tau [n-1]), the reflectors stay in A (vp_sym_tridiag)."""
+        assert A.dtype == torch.float64 and A.is_contiguous() and A.shape[0] == A.shape[1]
+        n = A.shape[0]
+        scratch = self.spectral_scratch(n) if scratch is None else scratch
+        d = torch.empty(n, dtype=torch.float64, device=self.device)
+        e = torch.empty(max(n - 1, 1), dtype=torch.float64, device=self.device)
+        tau = torch.empty(max(n - 1, 1), dtype=torch.float64, device=self.device)
+        _check(self._h, L.lib().vp_sym_tridiag(self._h, C.c_void_p(A.data_ptr()), n, C.c_void_p(d.data_ptr()),
+                                               C.c_void_p(e.data_ptr()), C.c_void_p(tau.data_ptr()),
+                                               C.c_void_p(scratch.data_ptr()), self.stream_ptr()))
+        return d, e[:n - 1], tau[:n - 1]
+
+    def sym_tridiag_apply_q(self, A, tau, Z):
+        """Z [n, k] (numpy / torch) -> device float64 Q Z with the reflectors sym_tridiag left in A, tau."""
+        tz = torch.as_tensor(Z, dtype=torch.float64).to(self.device).contiguous().clone()
+        n, k = tz.shape
+        tau_p = tau.data_ptr() if tau.numel() else A.data_ptr()
+        _check(self._h, L.lib().vp_sym_tridiag_apply_q(self._h, C.c_void_p(A.data_ptr()), C.c_void_p(tau_p), n,
+                                                       C.c_void_p(tz.data_ptr()), k, self.stream_ptr()))
+        return tz
+
+    def spectral_embedding(self, X, n_drop, n_eig, k_fn):
+        """SpectralCluster's spectral stage: embeddings X [n, D] -> (the n_eig smallest eigenvalues of the pruned-affinity
+        Laplacian, the eigenvectors of the first k = k_fn(eigenvalues) of them [n, k]), numpy float64.
+
+        Laplacian, Householder reduction and back-transformation run on the device in fp64; the tridiagonal
+        eigenproblem between them -- 2n numbers down, [n, k] up, O(n k) work -- is solved here by LAPACK's bisection and
+        inverse iteration (stebz / stein), which resolve clustered eigenvalues such as those of disconnected graph
+        components.  That split is by design, like k-means staying on the host; there is no CPU fallback for the O(n^3)
+        part."""
+        import scipy.linalg
+        n = len(X)
+        scratch = self.spectral_scratch(n)
+        A = self.spectral_laplacian(X, n_drop, scratch)
+        d, e, tau = self.sym_tridiag(A, scratch)
+        d, e = d.cpu().numpy(), e.cpu().numpy()
+        if n == 1:
+            lam = d.copy()
+            k = k_fn(lam)
+            return lam, np.ones((1, k))
+        lam = scipy.linalg.eigh_tridiagonal(d, e, eigvals_only=True, select='i', select_range=(0, n_eig - 1))
+        k = k_fn(lam)
+        _, Zt = scipy.linalg.eigh_tridiagonal(d, e, select='i', select_range=(0, k - 1))
+        return lam, self.sym_tridiag_apply_q(A, tau, Zt).cpu().numpy()
+
     def close(self):
         if self._h:
             for p in list(self._programs):

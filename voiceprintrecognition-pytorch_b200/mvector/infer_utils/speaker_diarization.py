@@ -10,7 +10,8 @@ the same interfaces, defaults and results as the reference classes:
                                       segments shorter than 1 s into a neighbour (:137-214)
   SpectralCluster                     cosine affinity -> keep the top p-fraction per row -> symmetrise -> unnormalised
                                       Laplacian -> eigengap (or oracle) speaker count -> k-means on the spectral
-                                      embedding (:217-310)
+                                      embedding (:217-310); MVectorPredictor runs everything up to the eigenvectors on
+                                      the device (csrc/spectral.cu, Engine.spectral_embedding)
 
 ``AudioSegment.vad`` (yeaudio's model-based VAD) is outside the parity boundary (SURVEY.md 8c); mvector.audio provides an
 energy-based stand-in with the same return format."""
@@ -25,10 +26,19 @@ class SpectralCluster:
         self.max_num_spks = max_num_spks
         self.pval = pval
 
-    sim_fn = None          # optional device scorer X -> [n, n] cosine matrix (MVectorPredictor installs vp_cosine_scores)
+    # Optional device implementation of the whole spectral stage (MVectorPredictor installs Engine.spectral_embedding):
+    #   spectral_fn(X [n, D] float32, n_drop, n_eig, k_fn) -> (the n_eig smallest Laplacian eigenvalues, their first
+    #   k = k_fn(eigenvalues) eigenvectors [n, k]).  None: everything below runs on the host, as in the reference.
+    spectral_fn = None
 
     def __call__(self, X, oracle_num=None):
-        sim = self.get_sim_mat(X) if self.sim_fn is None else np.array(self.sim_fn(np.asarray(X, dtype=np.float32)), dtype=np.float32)
+        if self.spectral_fn is not None:
+            n = len(X)
+            _, emb = self.spectral_fn(np.asarray(X, dtype=np.float32), self.n_drop(n), min(n, self.max_num_spks + 1),
+                                      lambda lambdas: self.num_speakers(lambdas, oracle_num))
+            # float32, the dtype the host path's (and the reference's) eigenvectors have: same k-means++ draws
+            return self.cluster_embs(np.asarray(emb, dtype=np.float32), emb.shape[1])
+        sim = self.get_sim_mat(X)
         affinity = self.p_pruning(sim)
         affinity = 0.5 * (affinity + affinity.T)
         emb, k = self.get_spec_embs(self.get_laplacian(affinity), oracle_num)
@@ -41,6 +51,12 @@ class SpectralCluster:
         n = np.linalg.norm(X, axis=1, keepdims=True)
         Xn = X / np.where(n == 0, 1, n)
         return Xn @ Xn.T
+
+    def n_drop(self, n):
+        """Entries p_pruning zeroes per row, as Python evaluates the reference's slice (a negative bound counts from
+        the end: n = 4 drops 2)."""
+        pval = 6.0 / n if n * self.pval < 6 else self.pval
+        return len(range(n)[:int((1 - pval) * n)])
 
     def p_pruning(self, A):
         """Zero all but the largest ceil-ish p-fraction of every row (at least 6 entries survive)."""
@@ -58,12 +74,15 @@ class SpectralCluster:
 
     def get_spec_embs(self, L, k_oracle=None):
         lambdas, vecs = scipy.linalg.eigh(L)
-        if k_oracle is not None:
-            k = k_oracle
-        else:
-            gaps = self.get_eigen_gaps(lambdas[self.min_num_spks - 1:self.max_num_spks + 1])
-            k = int(np.argmax(gaps)) + self.min_num_spks
+        k = self.num_speakers(lambdas, k_oracle)
         return vecs[:, :k], k
+
+    def num_speakers(self, lambdas, k_oracle=None):
+        """k_oracle, or the position of the largest gap among eigenvalues min_num_spks .. max_num_spks + 1."""
+        if k_oracle is not None:
+            return k_oracle
+        gaps = self.get_eigen_gaps(lambdas[self.min_num_spks - 1:self.max_num_spks + 1])
+        return int(np.argmax(gaps)) + self.min_num_spks
 
     @staticmethod
     def cluster_embs(emb, k):
@@ -83,9 +102,10 @@ class SpeakerDiarization(object):
         self.merge_threshold = merge_threshold
         self.spectral_cluster = SpectralCluster()
 
-    def set_similarity(self, sim_fn):
-        """Install a device scorer for the clustering's cosine affinity matrix (None: numpy on the host)."""
-        self.spectral_cluster.sim_fn = sim_fn
+    def set_spectral(self, spectral_fn):
+        """Install a device implementation of the clustering's spectral stage (SpectralCluster.spectral_fn; None: the
+        host path)."""
+        self.spectral_cluster.spectral_fn = spectral_fn
 
     # ------------------------------------------------------------------ segmentation
     def segments_audio(self, audio_segment):

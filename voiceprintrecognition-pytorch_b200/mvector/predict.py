@@ -8,8 +8,9 @@ Differences that are deliberate:
     the reference's ``batch_size`` argument (predict.py:261) is accepted and ignored -- chunking does not change
     results because every op is per-utterance, and padding/CMN/mask are computed on the full batch exactly like
     predict.py:244-258.
-  * ``speaker_diarization`` (predict.py:365-395): chunk embeddings come from ``predict_batch`` on the device; chunking,
-    spectral clustering and post-processing are host glue (infer_utils/speaker_diarization.py); the VAD is an energy
+  * ``speaker_diarization`` (predict.py:365-395): chunk embeddings come from ``predict_batch`` on the device, and
+    so does the spectral stage of the clustering up to its eigenvectors (``Engine.spectral_embedding``); chunking,
+    k-means and post-processing are host glue (infer_utils/speaker_diarization.py); the VAD is an energy
     detector standing in for yeaudio's model-based one (absent third-party code, outside the parity boundary).
 """
 import os
@@ -65,8 +66,9 @@ class MVectorPredictor:
         self._trace_dev = None
 
         self.speaker_diarize = SpeakerDiarization()
-        # similarity matrix of the spectral clustering (speaker_diarization.py:254-257) on the device
-        self.speaker_diarize.set_similarity(lambda X: self._engine.cosine_scores(X, X).cpu().numpy())
+        # spectral stage of the clustering (speaker_diarization.py:244-248: affinity, pruning, Laplacian, eigenvectors)
+        # on the device
+        self.speaker_diarize.set_spectral(self._engine.spectral_embedding)
 
         self.audio_feature = None
         self.audio_feature_mean = None
