@@ -1,5 +1,6 @@
-"""Op-level GPU tests of the two conv engines (exact fp32 FFMA, wgmma split-TF32) against the fp64 numpy interpreter
-(tests/plan_sim.py), over the conv geometries the five backbones use."""
+"""Op-level GPU tests of the two conv engines (exact fp32 FFMA, wgmma split-TF32) and of the pooling kernels against the
+fp64 numpy interpreter (tests/plan_sim.py), over the conv geometries the five backbones use and the input sizes on both
+sides of each pooling kernel choice."""
 import numpy as np
 import pytest
 import torch
@@ -200,3 +201,64 @@ def test_prologue_with_second_source_engine_ab(name):
     assert np.abs(got - ref).max() <= 2e-5 * max(1.0, np.abs(ref).max())
     with pytest.raises(L.VpError):
         _run_case(PRE_SRC2[name], L.ENGINE_TC)
+
+
+def _run_pool(case):
+    """One ASP_POOL (mean_only: SAP) or COLSTATS op on columns [coff, coff + C) (x) and [coff + C, coff + 2 C) (logits)
+    of a random input."""
+    from mvector import _lib as L
+    from mvector.engine import Engine, PlanBuilder, Program, View, WeightArena
+    from plan_sim import Sim
+    rng = np.random.default_rng(case['seed'])
+    B, R, C, coff = case['B'], case['R'], case['C'], case.get('coff', 0)
+    width = (coff + 2 * C + 3) // 4 * 4
+    X = (rng.standard_normal((B * R, width)) * 2).astype(np.float32)
+    arena = WeightArena()
+    arena.add('unused', np.zeros(4))
+    pb = PlanBuilder(B, L.ENGINE_AUTO)
+    pb.in_floats = B * R * width
+    inp = View(L.BUF_INPUT, width, 0, width)
+    x = inp.cols(coff, C)
+    if 'stats' in case:
+        mode = getattr(L, 'STATS_' + case['stats'])
+        seg_len = case.get('seg_len')
+        n_seg = -(-R // seg_len) if seg_len else 1
+        n_rows = B * n_seg
+        n_cols = C if mode in (L.STATS_MEAN, L.STATS_SEG_CONTEXT) else 2 * C
+        pb.colstats(x, pb.output_view(n_cols, n_rows), R, mode, eps=1e-5, seg_len=seg_len, n_seg=n_seg)
+    else:
+        n_rows, n_cols = B, C if case['mean_only'] else 2 * C
+        pb.asp_pool(x, inp.cols(coff + C, C), pb.output_view(n_cols, n_rows), R, eps=1e-12, mean_only=case['mean_only'])
+    eng = Engine()
+    blob = arena.blob()
+    eng.load_weights(blob)
+    y = torch.empty(n_rows, n_cols, device='cuda')
+    Program(eng, pb).run(torch.from_numpy(X).cuda().contiguous(), y)
+    torch.cuda.synchronize()
+    ref = Sim(pb, blob, X).run().reshape(n_rows, n_cols)
+    got = y.cpu().numpy()
+    eng.close()
+    return got, ref
+
+
+POOL_CASES = {}
+# ASP / mean-only SAP: the [T, 32] strips of x and logits are staged in shared memory up to T = 800 (T * 256 B <= 200 KB)
+for _T in (400, 401, 800, 801):
+    POOL_CASES[f'asp_T{_T}'] = dict(mean_only=False, B=3, R=_T, C=72, seed=_T)
+    POOL_CASES[f'sap_mean_T{_T}'] = dict(mean_only=True, B=3, R=_T, C=72, seed=_T + 1)
+# colstats: the [R, 32] strip is staged in shared memory up to R = 800 rows (R * 128 B <= 100 KB)
+for _i, _stats in enumerate(('MEAN', 'MEAN_STD_CLAMP', 'MEAN_STD_UNBIASED', 'MEAN_STD_TSTP', 'MEAN_VAR_UNBIASED')):
+    for _R in (800, 801):
+        POOL_CASES[f'colstats_{_stats.lower()}_R{_R}'] = dict(stats=_stats, B=3, R=_R, C=72, seed=_R + _i)
+# segment context: the segment sums are parked in shared memory up to 64 segments, two sweeps above
+for _n in (64, 65):
+    POOL_CASES[f'seg_context_{_n}'] = dict(stats='SEG_CONTEXT', B=3, R=10 * _n - 5, C=72, seg_len=10, seed=_n)
+# views that start one column into their matrix: no 16-byte staging, the global-memory kernels run
+POOL_CASES['asp_unaligned_coff'] = dict(mean_only=False, B=3, R=298, C=72, coff=1, seed=7)
+POOL_CASES['colstats_unaligned_coff'] = dict(stats='MEAN_STD_CLAMP', B=3, R=298, C=72, coff=1, seed=8)
+
+
+@pytest.mark.parametrize('name', list(POOL_CASES))
+def test_pool_kernels_match_interpreter(name):
+    got, ref = _run_pool(POOL_CASES[name])
+    assert np.abs(got - ref).max() <= 2e-5 * max(1.0, np.abs(ref).max())

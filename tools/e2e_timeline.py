@@ -61,14 +61,10 @@ torch.cuda.synchronize()
 print(f'H2D of {nbytes / 1e6:.1f} MB from pinned memory: {e0.elapsed_time(e1) / 5:.3f} ms = {nbytes * 5 / e0.elapsed_time(e1) / 1e6:.1f} GB/s')
 del hp, dp
 
-run(5)
-for fe_main in (True, False):
-    MVectorPredictor.FE_ON_MAIN = fe_main
-    run(3)
-    print(f'front-end on the {"main" if fe_main else "copy"} stream: per-call ms', [round(x, 2) for x in run(6, trace=True)])
-    ts = run(20)
-    print(f'   20 calls: median {np.median(ts):6.2f} ms  min {min(ts):6.2f}')
-MVectorPredictor.FE_ON_MAIN = os.environ.get('VPB_FE_STREAM', 'main') == 'main'
+run(8)
+print('per-call ms', [round(x, 2) for x in run(6, trace=True)])
+ts = run(20)
+print(f'   20 calls: median {np.median(ts):6.2f} ms  min {min(ts):6.2f}')
 if os.environ.get('VPB_TIMELINE_SWEEP', '1') == '0':
     sys.exit(0)
 for rows, sl, thr, mb in [(128, 8, 8, 256), (64, 8, 8, 256), (64, 16, 8, 256), (32, 8, 8, 256), (128, 8, 4, 256), (128, 4, 8, 256), (128, 16, 8, 256)]:

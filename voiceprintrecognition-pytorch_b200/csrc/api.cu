@@ -73,7 +73,7 @@ static int fail(vp_handle* h, int code, const char* fmt, ...) {
 static const int FPB = 16;   // frames per front-end CTA
 
 // VP_ENGINE_AUTO prefers the two-term FP16 split of the tensor-core engine where an op is eligible (conv_tc16_supported);
-// VPB_TC_F16=0 keeps AUTO on split TF32 (A/B runs).
+// VPB_TC_F16=0 keeps AUTO on split TF32, the bit-invariant reference engine.
 static bool tc16_enabled() {
   static int on = -1;
   if (on < 0) { const char* e = getenv("VPB_TC_F16"); on = (e && e[0] == '0') ? 0 : 1; }
@@ -645,13 +645,6 @@ static int run_ops(vp_program* p, const float* feats, float* emb, cudaStream_t s
   return VP_OK;
 }
 
-// VPB_GRAPH=0: always enqueue the ops one by one
-static bool graphs_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("VPB_GRAPH"); on = (e && e[0] == '0') ? 0 : 1; }
-  return on == 1;
-}
-
 // One vp_embed = one cudaGraphLaunch: the program's launches (tens for the TDNNs, hundreds for CAM++ / the 2-D nets) are
 // captured once per (feats, emb, arena) pointer triple on the handle's private stream -- the programmatic (PDL) edges
 // between the kernels are kept by the capture -- and replayed on the caller's stream.  The first run of a program is
@@ -695,7 +688,7 @@ static int embed_graph(vp_program* p, const float* feats, float* emb, cudaStream
 int vp_embed(vp_program* p, const float* feats, float* emb, void* stream) {
   if (!p || !feats || !emb) return p ? fail(p->h, VP_ERR_INVALID, "null argument") : VP_ERR_INVALID;
   CUDA_TRY(p->h, cudaSetDevice(p->h->device));
-  if (!graphs_enabled() || p->g_off || p->runs++ == 0) return run_ops(p, feats, emb, (cudaStream_t)stream, nullptr);
+  if (p->g_off || p->runs++ == 0) return run_ops(p, feats, emb, (cudaStream_t)stream, nullptr);
   return embed_graph(p, feats, emb, (cudaStream_t)stream);
 }
 

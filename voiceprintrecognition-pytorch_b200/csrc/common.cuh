@@ -37,7 +37,7 @@ struct PerDeviceSmem {
 __device__ __forceinline__ void pdl_launch_dependents() { asm volatile("griddepcontrol.launch_dependents;" ::: "memory"); }
 __device__ __forceinline__ void pdl_wait() { asm volatile("griddepcontrol.wait;" ::: "memory"); }
 
-// VPB_PDL=0 launches everything fully serialised (A/B runs)
+// VPB_PDL=0 launches everything fully serialised (per-kernel timing)
 inline int pdl_enabled() {
   static int on = -1;
   if (on < 0) { const char* e = getenv("VPB_PDL"); on = (e && e[0] == '0') ? 0 : 1; }

@@ -365,9 +365,7 @@ cudaError_t launch_conv_c1(const ConvParams& p, cudaStream_t stream) {
   // wide variant: N in {16, 32, 64}, <= 49 taps, epilogue = bias / act / affine / act2 only (what every stem uses)
   const bool plain = !p.ubias && !p.gate && !p.res && !p.sum && (p.N == 16 || p.N == 32 || p.N == 64) && p.KT * p.KF <= 49 &&
                      (p.out_ld & 3) == 0 && (p.out_coff & 3) == 0;
-  static int wide_pref = -1;
-  if (wide_pref < 0) { const char* e = getenv("VPB_C1_WIDE"); wide_pref = (e && e[0] == '0') ? 0 : 1; }
-  if (plain && wide_pref) {
+  if (plain) {
     const long long pairs = ((long long)p.M + 1) >> 1;
     long long blocks = (pairs + 255) / 256;
     if (blocks > 132 * 8) blocks = 132 * 8;

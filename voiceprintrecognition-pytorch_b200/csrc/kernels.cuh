@@ -77,10 +77,4 @@ cudaError_t launch_conv_tc(const ConvParams& p, cudaStream_t stream);
 bool conv_tc16_supported(const ConvParams& p);
 cudaError_t launch_conv_tc16(const ConvParams& p, const float* w_tc16, float descale, cudaStream_t stream);
 
-// opt-in experimental variants (pool_v2.cu, VPB_POOL_V2=1)
-bool asp_pool_v2_supported(const AspParams& p);
-cudaError_t launch_asp_pool_v2(const AspParams& p, cudaStream_t stream);
-bool colstats_v2_supported(const StatsParams& p);
-cudaError_t launch_colstats_v2(const StatsParams& p, cudaStream_t stream);
-
 }  // namespace vpb

@@ -4,36 +4,66 @@
 //                CAM++ StatsPool (campplus.py:27-33), TSTP (pooling.py:140-148), CAM++ context (campplus.py:96-111)
 //   asp_pool   : softmax over time + attentive mean/std (pooling.py:120-126)
 //   ew         : SE excite + residual (ecapa_tdnn.py:84,143; resnet_se.py:40-44), AFF blend (eres2net.py:48-50)
-#include <cstdlib>
-
 #include "kernels.cuh"
 
 namespace vpb {
+
+// Per-channel sum (or max) over the 8 warps of a 256-thread CTA with lane = channel; every thread gets its channel's
+// total.  Fixed order (warp 0, 1, ..., 7), so results are deterministic.  Ends on a barrier: the caller may reduce again
+// right away.
+__device__ __forceinline__ float block_reduce(float v, bool is_max) {
+  __shared__ float red[8][33];
+  __shared__ float bc[32];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  red[wid][lane] = v;
+  __syncthreads();
+  if (wid == 0) {
+    float s = red[0][lane];
+#pragma unroll
+    for (int i = 1; i < 8; ++i) s = is_max ? fmaxf(s, red[i][lane]) : s + red[i][lane];
+    bc[lane] = s;
+  }
+  __syncthreads();
+  const float r = bc[lane];
+  __syncthreads();
+  return r;
+}
+
+__device__ __forceinline__ void cp_async16(float* smem_dst, const float* gmem_src, bool valid) {
+  const unsigned dst = (unsigned)__cvta_generic_to_shared(smem_dst);
+  const int bytes = valid ? 16 : 0;                       // src-size 0: the 16 destination bytes are zero filled
+  asm volatile("cp.async.cg.shared.global [%0], [%1], 16, %2;" ::"r"(dst), "l"(gmem_src), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
+// Stage rows [0, R) of a [.., ld] matrix, 32 columns starting at column c0 (only columns < C are read; C % 4 == 0), into
+// dst[r * 32 + col]: 8 lanes x 16 B cover one 128-byte row, and every request of the CTA is in flight at once (one trip
+// to HBM instead of rounds of register-staged loads).
+__device__ __forceinline__ void stage_strip(float* dst, const float* src, int ld, int R, int c0, int C) {
+  const int c4 = (threadIdx.x & 7) * 4;
+  const bool cok = c0 + c4 < C;
+  const float* g = src + c0 + c4;
+  for (int r = threadIdx.x >> 3; r < R; r += blockDim.x >> 3)
+    cp_async16(dst + r * 32 + c4, cok ? g + (size_t)r * ld : src, cok);
+}
+
+// Second statistic of the non-segment colstats modes from the centred sum of squares.
+__device__ __forceinline__ float colstats_spread(const StatsParams& p, float ssq) {
+  if (p.mode == VP_STATS_MEAN_STD_CLAMP) return sqrtf(fmaxf(ssq / (float)p.R, p.eps));
+  if (p.mode == VP_STATS_MEAN_VAR_UNBIASED) return ssq / (float)(p.R - 1);
+  if (p.mode == VP_STATS_MEAN_STD_UNBIASED) return sqrtf(ssq / (float)(p.R - 1));
+  return sqrtf(ssq / (float)(p.R - 1) + p.eps);
+}
 
 // grid (ceil(C/32), B), block 256 = 8 warps; lane = channel, warps stride over the R rows.
 __global__ void __launch_bounds__(256) colstats_kernel(const __grid_constant__ StatsParams p) {
   pdl_launch_dependents();
   pdl_wait();                 // first access to mutable global memory comes after this
-  __shared__ float red[8][33];
-  __shared__ float bc[32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + lane;
   const int b = blockIdx.y;
   const bool ok = c < p.C;
   const float* x = p.src + (size_t)b * p.R * p.in_ld + p.in_coff + c;
-
-  auto block_sum = [&](float v) -> float {      // returns the per-channel total to every warp's lane
-    red[wid][lane] = v;
-    __syncthreads();
-    if (wid == 0) {
-      float s = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) s += red[i][lane];
-      bc[lane] = s;
-    }
-    __syncthreads();
-    return bc[lane];
-  };
 
   if (p.mode == VP_STATS_SEG_CONTEXT) {
     // context[b, s, c] = mean_T(x) + mean over segment s (last segment divides by its in-bounds length)
@@ -43,13 +73,12 @@ __global__ void __launch_bounds__(256) colstats_kernel(const __grid_constant__ S
       // utterance total first, then one segment at a time -- instead of parking the segment sums in shared memory
       float v = 0.f;
       if (ok) for (int r = wid; r < p.R; r += 8) v += x[(size_t)r * p.in_ld];
-      const float mean = block_sum(v) / (float)p.R;
+      const float mean = block_reduce(v, false) / (float)p.R;
       for (int s = 0; s < p.n_seg; ++s) {
         const int r0 = s * p.seg_len, r1 = min(r0 + p.seg_len, p.R);
         float u = 0.f;
         if (ok) for (int r = r0 + wid; r < r1; r += 8) u += x[(size_t)r * p.in_ld];
-        __syncthreads();
-        const float ss = block_sum(u);
+        const float ss = block_reduce(u, false);
         if (wid == 0 && ok) p.dst[((size_t)b * p.n_seg + s) * p.out_ld + p.out_coff + c] = mean + ss / (float)(r1 - r0);
       }
       return;
@@ -59,10 +88,9 @@ __global__ void __launch_bounds__(256) colstats_kernel(const __grid_constant__ S
       const int r0 = s * p.seg_len, r1 = min(r0 + p.seg_len, p.R);
       float v = 0.f;
       if (ok) for (int r = r0 + wid; r < r1; r += 8) v += x[(size_t)r * p.in_ld];
-      const float ss = block_sum(v);
+      const float ss = block_reduce(v, false);
       if (wid == 0) segsum[s][lane] = ss;
       total += ss;
-      __syncthreads();
     }
     if (wid == 0 && ok) {
       const float mean = total / (float)p.R;
@@ -76,70 +104,82 @@ __global__ void __launch_bounds__(256) colstats_kernel(const __grid_constant__ S
 
   float v = 0.f;
   if (ok) for (int r = wid; r < p.R; r += 8) v += x[(size_t)r * p.in_ld];
-  const float mean = block_sum(v) / (float)p.R;
+  const float mean = block_reduce(v, false) / (float)p.R;
   float* o = p.dst + (size_t)b * p.out_ld + p.out_coff;
   if (p.mode == VP_STATS_MEAN) {
     if (wid == 0 && ok) o[c] = mean;
     return;
   }
-  __syncthreads();
   float q = 0.f;
   if (ok) for (int r = wid; r < p.R; r += 8) { float d = x[(size_t)r * p.in_ld] - mean; q = fmaf(d, d, q); }
-  const float ssq = block_sum(q);
+  const float ssq = block_reduce(q, false);
   if (wid == 0 && ok) {
-    float sd;
-    if (p.mode == VP_STATS_MEAN_STD_CLAMP) sd = sqrtf(fmaxf(ssq / (float)p.R, p.eps));
-    else if (p.mode == VP_STATS_MEAN_VAR_UNBIASED) sd = ssq / (float)(p.R - 1);
-    else if (p.mode == VP_STATS_MEAN_STD_UNBIASED) sd = sqrtf(ssq / (float)(p.R - 1));
-    else sd = sqrtf(ssq / (float)(p.R - 1) + p.eps);
     o[c] = mean;
-    o[p.C + c] = sd;
+    o[p.C + c] = colstats_spread(p, ssq);
   }
 }
 
-// The supported shapes run on the cp.async one-trip staging kernels (pool_v2.cu: bit-identical results);
-// VPB_POOL_V2=0 keeps the register-staged kernels below for A/B runs.
-static bool pool_v2_enabled() {
-  static int on = -1;
-  if (on < 0) { const char* e = getenv("VPB_POOL_V2"); on = (e && e[0] == '0') ? 0 : 1; }
-  return on == 1;
+// The non-segment modes with the whole [R, 32] strip staged in shared memory (1-D maps): one trip to HBM, then the
+// same two-pass mean / centred sum of squares as colstats_kernel, out of shared memory.
+__global__ void __launch_bounds__(256) colstats_smem_kernel(const __grid_constant__ StatsParams p) {
+  pdl_launch_dependents();
+  pdl_wait();                 // first access to mutable global memory comes after this
+  extern __shared__ __align__(16) float sm[];
+  const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
+  const int c0 = blockIdx.x * 32;
+  const int c = c0 + lane;
+  const int b = blockIdx.y;
+  const bool ok = c < p.C;
+  stage_strip(sm, p.src + (size_t)b * p.R * p.in_ld + p.in_coff, p.in_ld, p.R, c0, p.C);
+  cp_async_wait_all();
+  __syncthreads();
+  float v = 0.f;
+  for (int r = wid; r < p.R; r += 8) v += sm[r * 32 + lane];
+  const float mean = block_reduce(v, false) / (float)p.R;
+  float* o = p.dst + (size_t)b * p.out_ld + p.out_coff;
+  if (p.mode == VP_STATS_MEAN) {
+    if (wid == 0 && ok) o[c] = mean;
+    return;
+  }
+  float q = 0.f;
+  for (int r = wid; r < p.R; r += 8) { float d = sm[r * 32 + lane] - mean; q = fmaf(d, d, q); }
+  const float ssq = block_reduce(q, false);
+  if (wid == 0 && ok) {
+    o[c] = mean;
+    o[p.C + c] = colstats_spread(p, ssq);
+  }
 }
 
 cudaError_t launch_colstats(const StatsParams& p, cudaStream_t stream) {
-  if (pool_v2_enabled() && colstats_v2_supported(p)) return launch_colstats_v2(p, stream);
   dim3 grid((p.C + 31) / 32, p.B);
+  const size_t smem = (size_t)p.R * 32 * sizeof(float);
+  // up to 100 KB of strip, so that two CTAs per SM keep loads and sweeps overlapped
+  if (p.mode != VP_STATS_SEG_CONTEXT && smem <= 100 * 1024 && (p.C & 3) == 0 && (p.in_ld & 3) == 0 && (p.in_coff & 3) == 0) {
+    static PerDeviceSmem once;
+    if (once.need(smem)) {
+      cudaError_t e = cudaFuncSetAttribute(colstats_smem_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, 100 * 1024);
+      if (e != cudaSuccess) return e;
+      once.set(100 * 1024);
+    }
+    launch_pdl(colstats_smem_kernel, grid, 256, smem, stream, p);
+    return cudaGetLastError();
+  }
   launch_pdl(colstats_kernel, grid, 256, 0, stream, p);
   return cudaGetLastError();
 }
 
 // Attentive statistics: alpha = softmax_t(logit[b, t, c]); mean = sum alpha x; std = sqrt(clamp(sum alpha (x-mean)^2, eps)).
 // x: src (in_ld/in_coff), logits: src2 (l_ld/l_coff); dst[b, c] = mean, dst[b, C + c] = std.
+// Reads x and logits from global memory in three sweeps (L2-resident): for T > 800 and unaligned views.
 __global__ void __launch_bounds__(256) asp_pool_kernel(const __grid_constant__ AspParams p) {
   pdl_launch_dependents();
   pdl_wait();                 // first access to mutable global memory comes after this
-  __shared__ float red[8][33];
-  __shared__ float bc[32];
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
   const int c = blockIdx.x * 32 + lane;
   const int b = blockIdx.y;
   const bool ok = c < p.C;
   const float* x = p.x + (size_t)b * p.T * p.x_ld + p.x_coff + c;
   const float* l = p.logit + (size_t)b * p.T * p.l_ld + p.l_coff + c;
-
-  auto block_reduce = [&](float v, bool is_max) -> float {
-    red[wid][lane] = v;
-    __syncthreads();
-    if (wid == 0) {
-      float s = red[0][lane];
-#pragma unroll
-      for (int i = 1; i < 8; ++i) s = is_max ? fmaxf(s, red[i][lane]) : s + red[i][lane];
-      bc[lane] = s;
-    }
-    __syncthreads();
-    float r = bc[lane];
-    __syncthreads();
-    return r;
-  };
 
   float mx = -INFINITY;
   if (ok) for (int t = wid; t < p.T; t += 8) mx = fmaxf(mx, l[(size_t)t * p.l_ld]);
@@ -167,64 +207,23 @@ __global__ void __launch_bounds__(256) asp_pool_kernel(const __grid_constant__ A
   }
 }
 
-// Same computation with the [T, 32-column] strips of x and logits staged ONCE in shared memory (each read from HBM once,
-// coalesced 128 B rows), then the three softmax / mean / variance sweeps run out of shared memory.
+// Same computation with the [T, 32-column] strips of x and logits staged once in shared memory (each read from HBM
+// once, coalesced 128 B rows), then the three softmax / mean / variance sweeps run out of shared memory.
 __global__ void __launch_bounds__(256) asp_pool_smem_kernel(const __grid_constant__ AspParams p) {
   pdl_launch_dependents();
   pdl_wait();                 // first access to mutable global memory comes after this
-  extern __shared__ float sm[];
-  __shared__ float red[8][33];
-  __shared__ float bc[32];
+  extern __shared__ __align__(16) float sm[];
   float* sx = sm;                       // [T][32]
   float* sl = sm + (size_t)p.T * 32;    // [T][32]
   const int lane = threadIdx.x & 31, wid = threadIdx.x >> 5;
-  const int c = blockIdx.x * 32 + lane;
+  const int c0 = blockIdx.x * 32;
+  const int c = c0 + lane;
   const int b = blockIdx.y;
   const bool ok = c < p.C;
-  {
-    // stage the strips: 8 lanes x float4 cover one 128-byte row, 32 rows per pass, 4 passes of loads in flight
-    const int c4 = (threadIdx.x & 7) * 4;
-    const int cc = blockIdx.x * 32 + c4;
-    const bool cok = cc < p.C;                      // C % 4 == 0 on this path (checked by the launcher)
-    const float* xb = p.x + (size_t)b * p.T * p.x_ld + p.x_coff + cc;
-    const float* lb = p.logit + (size_t)b * p.T * p.l_ld + p.l_coff + cc;
-    for (int t0 = threadIdx.x >> 3; t0 < p.T; t0 += 128) {
-      float4 xv[4], lv[4];
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int t = t0 + 32 * u;
-        xv[u] = make_float4(0.f, 0.f, 0.f, 0.f);
-        lv[u] = xv[u];
-        if (cok && t < p.T) {
-          xv[u] = __ldg(reinterpret_cast<const float4*>(xb + (size_t)t * p.x_ld));
-          lv[u] = __ldg(reinterpret_cast<const float4*>(lb + (size_t)t * p.l_ld));
-        }
-      }
-#pragma unroll
-      for (int u = 0; u < 4; ++u) {
-        const int t = t0 + 32 * u;
-        if (t < p.T) {
-          *reinterpret_cast<float4*>(sx + t * 32 + c4) = xv[u];
-          *reinterpret_cast<float4*>(sl + t * 32 + c4) = lv[u];
-        }
-      }
-    }
-  }
+  stage_strip(sx, p.x + (size_t)b * p.T * p.x_ld + p.x_coff, p.x_ld, p.T, c0, p.C);
+  stage_strip(sl, p.logit + (size_t)b * p.T * p.l_ld + p.l_coff, p.l_ld, p.T, c0, p.C);
+  cp_async_wait_all();
   __syncthreads();
-  auto block_reduce = [&](float v, bool is_max) -> float {
-    red[wid][lane] = v;
-    __syncthreads();
-    if (wid == 0) {
-      float s = red[0][lane];
-#pragma unroll
-      for (int i = 1; i < 8; ++i) s = is_max ? fmaxf(s, red[i][lane]) : s + red[i][lane];
-      bc[lane] = s;
-    }
-    __syncthreads();
-    float r = bc[lane];
-    __syncthreads();
-    return r;
-  };
   float mx = -INFINITY;
   for (int t = wid; t < p.T; t += 8) mx = fmaxf(mx, sl[t * 32 + lane]);
   mx = block_reduce(mx, true);
@@ -252,7 +251,6 @@ __global__ void __launch_bounds__(256) asp_pool_smem_kernel(const __grid_constan
 }
 
 cudaError_t launch_asp_pool(const AspParams& p, cudaStream_t stream) {
-  if (pool_v2_enabled() && asp_pool_v2_supported(p)) return launch_asp_pool_v2(p, stream);
   dim3 grid((p.C + 31) / 32, p.B);
   const size_t smem = (size_t)p.T * 32 * 2 * sizeof(float);
   if (smem <= 200 * 1024 && (p.C & 3) == 0 && (p.x_ld & 3) == 0 && (p.x_coff & 3) == 0 && (p.l_ld & 3) == 0 && (p.l_coff & 3) == 0) {

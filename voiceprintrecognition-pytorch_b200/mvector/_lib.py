@@ -4,7 +4,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-LIB_PATH = os.environ.get('VPB_LIB') or os.path.join(os.path.dirname(_HERE), 'libvpb200.so')   # VPB_LIB: dev builds (A/B runs)
+LIB_PATH = os.environ.get('VPB_LIB') or os.path.join(os.path.dirname(_HERE), 'libvpb200.so')   # VPB_LIB: dev builds
 
 VP_OK, VP_ERR_INVALID, VP_ERR_CUDA, VP_ERR_NOMEM, VP_ERR_UNSUPPORTED = 0, 1, 2, 3, 4
 OP_CONV, OP_CONV_C1, OP_COLSTATS, OP_ASP_POOL, OP_EW, OP_POOL2D = 1, 2, 3, 4, 5, 6

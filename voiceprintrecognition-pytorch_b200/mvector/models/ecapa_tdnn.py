@@ -26,9 +26,6 @@ def _tdnn_block_shapes(d, p, cin, cout, k):
     d[p + '.norm.norm.num_batches_tracked'] = ()
 
 
-RES2_SUM = os.environ.get('VPB_RES2_SUM', '0') == '1'      # dev knob while the two chain lowerings are compared
-
-
 def conv1d_weight(w):
     """[Cout, Cin, k] -> [Cout, k*Cin4] with K index = tap*Cin4 + ci (the gather order of the CONV op).  Cin4 = Cin
     rounded up to a multiple of 4 with zero columns: only a first layer fed by an odd feature dim (Spectrogram's
@@ -122,11 +119,10 @@ class EcapaTdnn(Backbone):
         o['fc_b'] = arena.add('fc.b', W @ h + _np64(sd['fc.conv.bias']))
 
     # ---- program ----
-    def _tdnn_block(self, pb, src, dst, w, T, k=1, dil=1, src2=None, sum_into=None):
+    def _tdnn_block(self, pb, src, dst, w, T, k=1, dil=1, src2=None):
         pad = dil * (k - 1) // 2
         pb.conv(src, dst, w['w'], k * src.C, T, T, KT=k, dT=dil, padT=pad, pad_mode=L.PAD_REFLECT, bias=w['b'],
-                act=L.ACT_RELU, post=(w['s'], w['h']), src2=src2, src2_mode=L.SRC2_ADD if src2 is not None else L.SRC2_NONE,
-                sum_into=sum_into)
+                act=L.ACT_RELU, post=(w['s'], w['h']), src2=src2, src2_mode=L.SRC2_ADD if src2 is not None else L.SRC2_NONE)
 
     def _lower(self, pb, B, T):
         ch, ks, dl = self.channels, self.kernel_sizes, self.dilations
@@ -151,18 +147,13 @@ class EcapaTdnn(Backbone):
             self._tdnn_block(pb, xin, t1, blk['tdnn1'], T)
             y = pb.alloc(M, c)
             pb.ew(L.EW_COPY, t1.cols(0, w), y.cols(0, w), T)
-            # Res2Net chain (ecapa_tdnn.py Res2NetBlock.forward): y_j = block_j(x_j + y_{j-1}).
-            #   default: the add rides in conv j's gather as a second source (two loads per element);
-            #   VPB_RES2_SUM=1: conv j-1's epilogue adds y_{j-1} into x_j in place (vp_op.sum) and conv j gathers ONE
-            #   source.  Parity-green; off by default because the read-modify-write lengthens the epilogue, which at a
-            #   few tiles per CTA is exposed at every tile hand-over.
+            # Res2Net chain (ecapa_tdnn.py Res2NetBlock.forward): y_j = block_j(x_j + y_{j-1}).  The add rides in conv
+            # j's gather as a second source (two loads per element), not in conv j-1's epilogue as an in-place add
+            # (vp_op.sum): that read-modify-write lengthens the epilogue, which at a few tiles per CTA is exposed at every
+            # tile hand-over.
             for j in range(1, sc):
-                if RES2_SUM:
-                    self._tdnn_block(pb, t1.cols(j * w, w), y.cols(j * w, w), blk['res2'][j - 1], T, ks[i], dl[i],
-                                     sum_into=t1.cols((j + 1) * w, w) if j + 1 < sc else None)
-                else:
-                    self._tdnn_block(pb, t1.cols(j * w, w), y.cols(j * w, w), blk['res2'][j - 1], T, ks[i], dl[i],
-                                     src2=y.cols((j - 1) * w, w) if j >= 2 else None)
+                self._tdnn_block(pb, t1.cols(j * w, w), y.cols(j * w, w), blk['res2'][j - 1], T, ks[i], dl[i],
+                                 src2=y.cols((j - 1) * w, w) if j >= 2 else None)
             pb.free(t1)
             t2 = pb.alloc(M, c)
             self._tdnn_block(pb, y, t2, blk['tdnn2'], T)

@@ -183,28 +183,24 @@ class MVectorPredictor:
         return audio_segment
 
     #: utterances per backbone program (one fused vp_embed per chunk); the workspace limit can lower it for big 2-D nets
-    MAX_BATCH = int(os.environ.get('VPB_PREDICT_CHUNK', '256'))
+    MAX_BATCH = 256
     #: utterances per staging call (host gather -> pinned -> H2D -> front-end kernels), double buffered
-    STAGE_ROWS = int(os.environ.get('VPB_STAGE_ROWS', '128'))
+    STAGE_ROWS = 128
     #: utterances per H2D copy inside a staging call (the copy of slice k overlaps the gather of slice k+1)
-    COPY_SLICE = int(os.environ.get('VPB_COPY_SLICE', '4'))
+    COPY_SLICE = 4
     #: utterances per backbone program on the HOST-staged path: smaller than MAX_BATCH so that the backbone of chunk k runs
     #: while the host gathers and copies chunk k+1
-    HOST_CHUNK = int(os.environ.get('VPB_HOST_CHUNK', '128'))
-    #: front-end kernels on the main stream right before their backbone chunk ('main'), or on the copy stream behind their
-    #: data ('copy': there they sit between two stages' H2D copies and hold the second one up)
-    FE_ON_MAIN = os.environ.get('VPB_FE_STREAM', 'main') == 'main'
-    #: staging gather with non-temporal stores: '1' / '0', or 'auto' = only when several ranks share this host (their
-    #: gathers run at the same time and are DRAM-bound; the single-process path keeps the measured memcpy gather)
-    GATHER_NT = os.environ.get('VPB_GATHER_NT', 'auto')
+    HOST_CHUNK = 128
     _gather_configured = False
     #: program workspace cap: leaves an 80 GB H100 room for weights, inputs and the caller's own tensors
     WS_LIMIT_BYTES = int(float(os.environ.get('VPB_WS_LIMIT_GB', '48')) * 2 ** 30)
 
     @classmethod
     def _configure_gather(cls, lib):
+        """Staging gather with non-temporal stores only when several ranks share this host: their gathers run at the same
+        time and are DRAM-bound, while the single-process path keeps the measured memcpy gather."""
         if not cls._gather_configured:
-            on = cls.GATHER_NT == '1' or (cls.GATHER_NT == 'auto' and int(os.environ.get('LOCAL_WORLD_SIZE', '1')) > 1)
+            on = int(os.environ.get('LOCAL_WORLD_SIZE', '1')) > 1
             lib.vp_host_gather_streaming(1 if on else 0)
             cls._gather_configured = True
 
@@ -305,7 +301,7 @@ class MVectorPredictor:
         slices finish (``vp_host_stage_h2d``) -- feed the fused front-end kernels, which run on the main stream behind an
         event of their stage's copies and write straight into the [B, T, F] feature buffer; as soon as the features of a
         backbone chunk (``_host_chunks``) are complete the main stream runs its program, under the next stage's gather and
-        copies.  One D2H of the result at the end.  (``VPB_FE_STREAM=copy``: front-end kernels on the copy stream.)"""
+        copies.  One D2H of the result at the end."""
         from . import _lib as L
         import ctypes as C
         import time
@@ -337,8 +333,7 @@ class MVectorPredictor:
         whole = desc.post == 1 and desc.top_db >= 0      # MFCC: the top_db clamp needs the maximum over the whole call
         S = B if whole else min(self.STAGE_ROWS, B)
         nstages = (B + S - 1) // S
-        fe_main = self.FE_ON_MAIN
-        K = min(nstages, 4 if fe_main else 2)           # device staging slots (the pinned side always has two)
+        K = min(nstages, 4)                             # device staging slots (the pinned side always has two)
         dwave = torch.empty(K, S * lmax, dtype=torch.float32, device=dev)
         scratch = torch.empty(max(int(lib.vp_frontend_scratch_floats(eng.handle, S, lmax)), 1), dtype=torch.float32, device=dev)
         if self._copy_stream is None:
@@ -346,8 +341,7 @@ class MVectorPredictor:
         cs = self._copy_stream
         cs_ptr = C.c_void_p(cs.cuda_stream)
         main = torch.cuda.current_stream(dev)
-        fs = main if fe_main else cs                    # stream of the front-end kernels
-        fs_ptr = C.c_void_p(fs.cuda_stream)
+        main_ptr = C.c_void_p(main.cuda_stream)
         cs.wait_stream(main)                            # buffers handed out by the allocator may still be in use on main
         ptrs = np.empty(B, dtype=np.uint64)              # filled stage by stage: only stage 0's part is on the critical path
         lens = np.fromiter(map(len, waves), dtype=np.int32, count=B)
@@ -386,24 +380,21 @@ class MVectorPredictor:
             cev.record(cs)
             pin_ev[ps] = cev
             dmark(f'stage {gi}: H2D done', cs)
-            if fe_main:
-                main.wait_event(cev)
+            main.wait_event(cev)
             kp = C.c_void_p(keep_all.data_ptr() + 4 * g0) if keep_all is not None else C.c_void_p()
             if whole and group is not None:
-                fz.mfcc_sharded(dw, n, lmax, kp, feats, scratch, fs, group)
+                fz.mfcc_sharded(dw, n, lmax, kp, feats, scratch, main, group)
             else:
                 from .engine import _check
                 _check(eng.handle, fe_fn(eng.handle, C.c_void_p(dw.data_ptr()), n, lmax, kp,
-                                         C.c_void_p(feats.data_ptr() + 4 * g0 * T * F), C.c_void_p(scratch.data_ptr()), fs_ptr))
+                                         C.c_void_p(feats.data_ptr() + 4 * g0 * T * F), C.c_void_p(scratch.data_ptr()), main_ptr))
             fev = torch.cuda.Event()
-            fev.record(fs)
+            fev.record(main)
             dev_ev[ds] = fev
-            dmark(f'stage {gi}: front-end done', fs)
+            dmark(f'stage {gi}: front-end done', main)
             # backbone chunks whose features are now complete
             while bounds and bounds[0] <= g1:
                 hi = bounds.pop(0)
-                if not fe_main:
-                    main.wait_event(fev)
                 self.predictor.program(hi - next_chunk, T).run(feats[next_chunk:hi], emb[next_chunk:hi])
                 dmark(f'backbone rows {next_chunk}:{hi} done', main)
                 next_chunk = hi
