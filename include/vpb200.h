@@ -258,6 +258,45 @@ int vp_sym_tridiag_apply_q(vp_handle* h, const double* A, const double* tau, int
 /* kernel launches of one vp_spectral_laplacian + vp_sym_tridiag + vp_sym_tridiag_apply_q at size n */
 int32_t vp_spectral_launches(int32_t n);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Verification metrics of MVectorTrainer.evaluate (trainer.py:462-468, metric/metrics.py:5-39) on the device: EER,
+ * minDCF and the EER threshold of n scores, without copying the scores or building a label matrix on the host.
+ * With order = argsort(scores, kind='stable') and T_i / I_i the inclusive counts of targets (label 1) / impostors
+ * (label 0) among the first i+1 sorted scores, T = T_{n-1}, I = I_{n-1}:
+ *   fnr[i] = T_i / T,  fpr[i] = 1 - I_i / I,  gap[i] = fnr[i] - fpr[i],
+ *   cost[i] = ((c_miss * fnr[i]) * p_target) + ((c_fa * fpr[i]) * (1 - p_target))
+ * in float64 with every operation rounded on its own (no FMA) -- the values numpy's compute_fnr_fpr / compute_dcf form.
+ * Equal scores keep their index order (stable sort; the reference's default quicksort leaves that order open); -0 sorts
+ * as +0 and every NaN after +inf, as numpy sorts them.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct vp_verify_result {
+  int64_t n_target;        /* T: scores with label 1 */
+  int64_t n_impostor;      /* I: scores with label 0 (any other flat label counts as neither) */
+  int64_t x1;              /* first sorted index with gap >= 0, -1 if none (compute_eer's x1) */
+  int64_t x2;              /* last sorted index with gap < 0, -1 if none (compute_eer's x2) */
+  int64_t target_x1;       /* T_{x1} (0 if x1 = -1) */
+  int64_t impostor_x1;     /* I_{x1} */
+  int64_t target_x2;       /* T_{x2} (0 if x2 = -1) */
+  int64_t impostor_x2;     /* I_{x2} */
+  double  min_cost;        /* min over i of cost[i] (compute_dcf's c_det before the division by c_def) */
+  int64_t argmin;          /* first index attaining min_cost, -1 if n = 0 */
+  float   threshold;       /* sorted score at x1 (compute_eer's threshold; NaN if x1 = -1) */
+  int32_t reserved0;
+} vp_verify_result;
+/* device scratch bytes vp_verify_metrics needs for n scores: about 10.3 bytes per score */
+size_t vp_verify_scratch_bytes(const vp_handle* h, int64_t n);
+/* scores [n] float32 (device, caller-owned; not modified), 0 <= n <= 2^31, and EITHER labels [n] int32 (flat form, as
+ * compute_fnr_fpr takes them: 1 target, 0 impostor) with trial_labels = enroll_labels = NULL, OR labels = NULL and
+ * trial_labels [n_trials] / enroll_labels [n_enroll] int32 with n = n_trials * n_enroll: score i is trial i / n_enroll
+ * against enrolment i % n_enroll and a target iff their labels are equal (evaluate's trial-major matrix).
+ * sorted_scores [n] float32 / sorted_labels [n] uint8 (1 target, 0 impostor, 2 neither) receive the sorted sequence
+ * when not NULL.  result: DEVICE pointer to one vp_verify_result, valid once the stream reaches the end of the call.
+ * All launches are asynchronous; no floating-point atomics: two calls give bit-identical results. */
+int vp_verify_metrics(vp_handle* h, const float* scores, int64_t n, const int32_t* labels, const int32_t* trial_labels,
+                      int64_t n_trials, const int32_t* enroll_labels, int64_t n_enroll, double p_target, double c_miss,
+                      double c_fa, void* scratch, float* sorted_scores, uint8_t* sorted_labels, vp_verify_result* result,
+                      void* stream);
+
 /* Staging half of predict_batch (predict.py:244-255) as ONE native call: worker threads gather slices of slice_rows
  * utterances into the zero-padded PINNED matrix staging[n, lmax]; the calling thread -- one of the n_threads gatherers --
  * issues cudaMemcpyAsync(staging slice -> device_dst slice) on copy_stream, in slice order, as soon as a slice is

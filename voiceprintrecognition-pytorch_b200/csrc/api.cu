@@ -794,6 +794,35 @@ int vp_sym_tridiag_apply_q(vp_handle* h, const double* A, const double* tau, int
 
 int32_t vp_spectral_launches(int32_t n) { return n < 1 ? 0 : spectral_launches_laplacian() + spectral_launches_tridiag(n) + 1; }
 
+size_t vp_verify_scratch_bytes(const vp_handle* h, int64_t n) {
+  (void)h;
+  return n < 0 || n > ((int64_t)1 << 31) ? 0 : verify_scratch_bytes(n);
+}
+
+int vp_verify_metrics(vp_handle* h, const float* scores, int64_t n, const int32_t* labels, const int32_t* trial_labels,
+                      int64_t n_trials, const int32_t* enroll_labels, int64_t n_enroll, double p_target, double c_miss,
+                      double c_fa, void* scratch, float* sorted_scores, uint8_t* sorted_labels, vp_verify_result* result,
+                      void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (!result || !scratch || (n > 0 && !scores)) return fail(h, VP_ERR_INVALID, "null argument");
+  if (n < 0 || n > ((int64_t)1 << 31)) return fail(h, VP_ERR_UNSUPPORTED, "n = %lld outside [0, 2^31]", (long long)n);
+  const bool flat = labels != nullptr, matrix = trial_labels != nullptr || enroll_labels != nullptr;
+  if (flat == matrix) return fail(h, VP_ERR_INVALID, "pass either labels or trial_labels + enroll_labels");
+  if (matrix) {
+    if (!trial_labels || !enroll_labels || n_trials < 0 || n_enroll < 0)
+      return fail(h, VP_ERR_INVALID, "matrix form needs trial_labels and enroll_labels");
+    if (n_trials * n_enroll != n)
+      return fail(h, VP_ERR_INVALID, "n = %lld != n_trials * n_enroll = %lld * %lld", (long long)n, (long long)n_trials,
+                  (long long)n_enroll);
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  if (n > 0)
+    CUDA_TRY(h, launch_verify_sort(scores, labels, trial_labels, enroll_labels, n_enroll, n, scratch, (cudaStream_t)stream));
+  CUDA_TRY(h, launch_verify_curve(n, p_target, c_miss, c_fa, scratch, sorted_scores, sorted_labels, result,
+                                  (cudaStream_t)stream));
+  return VP_OK;
+}
+
 int vp_program_peek(vp_program* p, int64_t off, size_t nbytes, void* dst, void* stream) {
   if (!p || !dst) return VP_ERR_INVALID;
   if (off < 0 || (size_t)off + nbytes > p->ws_bytes) return fail(p->h, VP_ERR_INVALID, "peek out of range");

@@ -60,6 +60,13 @@ cudaError_t launch_spectral_laplacian(const float* emb, int n, int D, int n_drop
 cudaError_t launch_sym_tridiag(double* A, int n, double* d, double* e, double* tau, void* scratch, cudaStream_t stream);
 cudaError_t launch_sym_tridiag_apply_q(const double* A, const double* tau, int n, double* Z, int kz, cudaStream_t stream);
 
+// verification metrics: stable radix sort of the scores + fp64 miss / false-alarm curves (verify.cu)
+size_t verify_scratch_bytes(int64_t n);
+cudaError_t launch_verify_sort(const float* scores, const int32_t* labels, const int32_t* trial, const int32_t* enroll,
+                               int64_t n_enroll, int64_t n, void* scratch, cudaStream_t stream);
+cudaError_t launch_verify_curve(int64_t n, double p_target, double c_miss, double c_fa, void* scratch, float* sorted_scores,
+                                uint8_t* sorted_labels, vp_verify_result* result, cudaStream_t stream);
+
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);

@@ -40,6 +40,12 @@ class Op(C.Structure):
                    ('w_tc16_q', C.c_int32), ('tc16_descale', C.c_float), ('amax_out', C.c_int32), ('amax_in', C.c_int32), ('tc_kc', C.c_int32), ('reserved0', C.c_int32)])
 
 
+class VerifyResult(C.Structure):
+    _fields_ = ([(n, C.c_int64) for n in ('n_target', 'n_impostor', 'x1', 'x2', 'target_x1', 'impostor_x1', 'target_x2',
+                                          'impostor_x2')]
+                + [('min_cost', C.c_double), ('argmin', C.c_int64), ('threshold', C.c_float), ('reserved0', C.c_int32)])
+
+
 class VpError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f'vpb200 error {code}: {msg}')
@@ -96,6 +102,9 @@ def lib():
         'vp_sym_tridiag': (C.c_int, [vp, C.c_void_p, i32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, vp]),
         'vp_sym_tridiag_apply_q': (C.c_int, [vp, C.c_void_p, C.c_void_p, i32, C.c_void_p, i32, vp]),
         'vp_spectral_launches': (i32, [i32]),
+        'vp_verify_scratch_bytes': (sz, [vp, C.c_int64]),
+        'vp_verify_metrics': (C.c_int, [vp, f32p, C.c_int64, i32p, i32p, C.c_int64, i32p, C.c_int64, C.c_double,
+                                        C.c_double, C.c_double, C.c_void_p, f32p, C.c_void_p, C.c_void_p, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = header/library mismatch
@@ -116,4 +125,4 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_program_launches', 'vp_program_peek', 'vp_embed_profiled', 'vp_program_op_info', 'vp_host_gather_pad',
            'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_cosine_scores', 'vp_device_zero',
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
-           'vp_spectral_launches']
+           'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics']

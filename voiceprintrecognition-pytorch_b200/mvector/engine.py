@@ -125,6 +125,48 @@ class Engine:
         _, Zt = scipy.linalg.eigh_tridiagonal(d, e, select='i', select_range=(0, k - 1))
         return lam, self.sym_tridiag_apply_q(A, tau, Zt).cpu().numpy()
 
+    # ---- verification metrics (csrc/verify.cu) ----
+    def verify(self, scores, labels=None, trial_labels=None, enroll_labels=None, p_target=0.01, c_miss=1, c_fa=1,
+               sorted_out=False):
+        """vp_verify_metrics on a flat score list: -> (vp_verify_result, sorted scores, sorted label codes), the last
+        two device tensors with ``sorted_out`` else None.  Labels: ``labels`` [n] (flat form) or ``trial_labels`` /
+        ``enroll_labels`` with n = n_trials * n_enroll, score i = trial i // n_enroll against enrolment i % n_enroll."""
+        ts = torch.as_tensor(scores, dtype=torch.float32).to(self.device).contiguous().reshape(-1)
+        n = ts.numel()
+
+        def dev_i32(x):
+            return None if x is None else torch.as_tensor(np.asarray(x), dtype=torch.int32).to(self.device).contiguous().reshape(-1)
+
+        tl, tt, te = dev_i32(labels), dev_i32(trial_labels), dev_i32(enroll_labels)
+        if tl is not None and tl.numel() != n:
+            raise ValueError(f'{n} scores but {tl.numel()} labels')
+        def ptr(t):                    # NULL for an absent tensor; an empty label vector still selects its form
+            return C.c_void_p(None if t is None else (t.data_ptr() or 1))
+
+        scratch = torch.empty(max(int(L.lib().vp_verify_scratch_bytes(self._h, n)), 1), dtype=torch.uint8,
+                              device=self.device)
+        res_dev = torch.empty(C.sizeof(L.VerifyResult), dtype=torch.uint8, device=self.device)
+        ss = torch.empty(n, dtype=torch.float32, device=self.device) if sorted_out else None
+        sl = torch.empty(n, dtype=torch.uint8, device=self.device) if sorted_out else None
+        _check(self._h, L.lib().vp_verify_metrics(
+            self._h, ptr(ts), n, ptr(tl), ptr(tt), 0 if tt is None else tt.numel(), ptr(te),
+            0 if te is None else te.numel(), float(p_target), float(c_miss), float(c_fa), C.c_void_p(scratch.data_ptr()),
+            ptr(ss), ptr(sl), C.c_void_p(res_dev.data_ptr()), self.stream_ptr()))
+        res = L.VerifyResult.from_buffer_copy(res_dev.cpu().numpy().tobytes())      # the one synchronise
+        return res, ss, sl
+
+    def verification_metrics(self, scores_dev, labels=None, trial_labels=None, enroll_labels=None, p_target=0.01,
+                             c_miss=1, c_fa=1, curves=False):
+        """EER / minDCF / threshold of a score list on the device (compute_fnr_fpr + compute_eer + compute_dcf,
+        metric/metrics.py) -> (eer, min_dcf, threshold), plus (fnr, fpr, thresholds) numpy arrays with ``curves``.
+        Raises IndexError where compute_eer does."""
+        from .metric.verification import curves_from_sorted, metrics_from_result
+        res, ss, sl = self.verify(scores_dev, labels, trial_labels, enroll_labels, p_target, c_miss, c_fa, curves)
+        out = metrics_from_result(res, p_target, c_miss, c_fa)
+        if not curves:
+            return out
+        return out + curves_from_sorted(ss.cpu().numpy(), sl.cpu().numpy())
+
     def close(self):
         if self._h:
             for p in list(self._programs):

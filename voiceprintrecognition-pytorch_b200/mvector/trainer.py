@@ -13,8 +13,10 @@ kernel.
 duration (``np.argsort``), every file is featurized ALONE (CMN over its own frames, no mask), cropped from the start to
 ``eval_conf.max_duration``, then ``eval_conf.batch_size`` consecutive features are zero-padded at the FEATURE level to
 the longest in the batch and fed to the backbone -- padded frames do reach the pooling layer, exactly as in the
-reference.  Front-end and backbone run on the sm_90a kernels; the score matrix / EER / minDCF are numpy glue
-(trainer.py:452-468, metric/metrics.py).  Training and export are outside the embedding-extraction path and raise."""
+reference.  Front-end, backbone and cosine scores run on the sm_90a kernels.  EER / minDCF (trainer.py:462-468,
+metric/metrics.py) run on the device too once the score matrix has ``DEVICE_METRICS_MIN`` entries (csrc/verify.cu: a
+stable radix sort of the scores and exact fp64 curves; no score copy, no host label matrix); smaller matrices take the
+numpy glue.  Training and export are outside the embedding-extraction path and raise."""
 import os
 import time
 
@@ -30,6 +32,9 @@ from .utils.utils import dict_to_object, print_arguments
 
 
 class MVectorTrainer(object):
+    # score-matrix size (n_trials * n_enroll) from which evaluate computes EER / minDCF on the device (DESIGN.md 8.2)
+    DEVICE_METRICS_MIN = 1 << 20
+
     def __init__(self, configs, use_gpu=True, data_augment_configs=None):
         if use_gpu:
             assert torch.cuda.is_available(), 'GPU不可用'
@@ -193,11 +198,19 @@ class MVectorTrainer(object):
             return -1, -1, -1
         logger.info('开始对比音频特征...')
         # cosine_similarity of every trial against every enrolment (trainer.py:454-461), trial-major order, on the device
-        all_score = self._cosine_scores(trials_features, enroll_features).reshape(-1)
-        all_labels = (trials_labels[:, None] == enroll_labels[None, :]).astype(np.int32).reshape(-1)
-        fnr, fpr, thresholds = compute_fnr_fpr(all_score, all_labels)
-        eer, threshold = compute_eer(fnr, fpr, all_score)
-        min_dcf = compute_dcf(fnr, fpr)
+        if len(trials_labels) * len(enroll_labels) >= self.DEVICE_METRICS_MIN:
+            scores = self._engine.cosine_scores(trials_features, enroll_features)
+            out = self._engine.verification_metrics(scores.reshape(-1), trial_labels=trials_labels,
+                                                    enroll_labels=enroll_labels, curves=bool(save_image_path))
+            eer, min_dcf, threshold = out[:3]
+            if save_image_path:
+                fnr, fpr, thresholds = out[3:]
+        else:
+            all_score = self._cosine_scores(trials_features, enroll_features).reshape(-1)
+            all_labels = (trials_labels[:, None] == enroll_labels[None, :]).astype(np.int32).reshape(-1)
+            fnr, fpr, thresholds = compute_fnr_fpr(all_score, all_labels)
+            eer, threshold = compute_eer(fnr, fpr, all_score)
+            min_dcf = compute_dcf(fnr, fpr)
         eer, min_dcf, threshold = float(eer), float(min_dcf), float(threshold)
         if save_image_path:                                                       # trainer.py:471-484
             import matplotlib.pyplot as plt
