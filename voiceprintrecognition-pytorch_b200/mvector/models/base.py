@@ -22,6 +22,26 @@ def bn_affine(sd, prefix, eps=1e-5):
     return s, beta - mean * s
 
 
+def bn_names(d, p, c, affine=True):
+    if affine:
+        d[p + '.weight'] = (c,)
+        d[p + '.bias'] = (c,)
+    d[p + '.running_mean'] = (c,)
+    d[p + '.running_var'] = (c,)
+    d[p + '.num_batches_tracked'] = ()
+
+
+def conv1d_weight(w):
+    """[Cout, Cin, k] -> [Cout, k*Cin4] with K index = tap*Cin4 + ci (the gather order of the CONV op).  Cin4 = Cin
+    rounded up to a multiple of 4 with zero columns: only a first layer fed by an odd feature dim (Spectrogram's
+    n_fft/2+1 bins) is ever padded; its input comes through PlanBuilder.input_view1d."""
+    w = _np64(w)
+    cin = w.shape[1]
+    if cin % 4:
+        w = np.concatenate([w, np.zeros((w.shape[0], -cin % 4, w.shape[2]), dtype=w.dtype)], axis=1)
+    return np.ascontiguousarray(w.transpose(0, 2, 1)).reshape(w.shape[0], -1)
+
+
 class Backbone:
     """Base of the model mirrors.  A backbone is *lowered* for a concrete (B, T) into a vp_program; programs are
     cached per shape.  Calling the object runs features [B, T, F] (CUDA fp32) -> embeddings [B, embd_dim]."""

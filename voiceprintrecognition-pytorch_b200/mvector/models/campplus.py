@@ -12,12 +12,10 @@
 import math
 from collections import OrderedDict
 
-import numpy as np
-
 from .. import _lib as L
-from .base import Backbone, _np64, bn_affine
-from .conv2d_util import bn_names, conv2d_weight, fc_perm, fold_conv_bn, out_len
-from .ecapa_tdnn import conv1d_weight
+from ..engine import View
+from .base import Backbone, _np64, bn_affine, bn_names, conv1d_weight
+from .conv2d_util import fc_perm, lower_stem_c1, out_len, pack_conv_bn
 
 _BLOCKS = ((12, 3, 1), (24, 3, 2), (16, 3, 2))
 _SEG = 100
@@ -78,21 +76,15 @@ class CAMPPlus(Backbone):
 
     def _pack(self, sd, arena):
         o = self._off
-
-        def cb(name, conv_key, bn):
-            W, b = fold_conv_bn(sd, conv_key, bn)
-            o[name] = dict(w=arena.add_conv(name + '.w', W), b=arena.add(name + '.b', b))
-
-        W, b = fold_conv_bn(sd, 'head.conv1.weight', 'head.bn1')        # [32, (kt,kf,1)] -> 9 taps
-        o['stem'] = dict(w=arena.add('stem.w', W), b=arena.add('stem.b', b))
+        pack_conv_bn(sd, arena, o, 'stem', 'head.conv1.weight', 'head.bn1')
         for layer in ('layer1', 'layer2'):
             for bi in range(2):
                 p = f'head.{layer}.{bi}'
-                cb(p + '.c1', p + '.conv1.weight', p + '.bn1')
-                cb(p + '.c2', p + '.conv2.weight', p + '.bn2')
+                pack_conv_bn(sd, arena, o, p + '.c1', p + '.conv1.weight', p + '.bn1')
+                pack_conv_bn(sd, arena, o, p + '.c2', p + '.conv2.weight', p + '.bn2')
                 if bi == 0:
-                    cb(p + '.sc', p + '.shortcut.0.weight', p + '.shortcut.1')
-        cb('head.c2', 'head.conv2.weight', 'head.bn2')
+                    pack_conv_bn(sd, arena, o, p + '.sc', p + '.shortcut.0.weight', p + '.shortcut.1')
+        pack_conv_bn(sd, arena, o, 'head.c2', 'head.conv2.weight', 'head.bn2')
         # TDNN layer: K columns (kt, f*32+c) <- reference channel c*F8+f
         perm = fc_perm(self.F8, self.m)
         Wt = _np64(sd['xvector.tdnn.linear.weight'])[:, perm, :]             # [N, mycol, kt]
@@ -124,13 +116,8 @@ class CAMPPlus(Backbone):
 
     def _lower(self, pb, B, T):
         o, m = self._off, self.m
-        F = self.input_size
-        x_in = pb.input_view(F, B * T)
         # ---- FCM head ----
-        x = pb.alloc(B * T * F, m)
-        pb.conv(L_view1(x_in), x, o['stem']['w'], 9, T, T, Fin=F, Fout=F, KT=3, KF=3, padT=1, padF=1,
-                bias=o['stem']['b'], act=L.ACT_RELU, c1=True)
-        f = F
+        x, _, f = lower_stem_c1(pb, o['stem'], B, T, self.input_size, m)
         for layer in ('layer1', 'layer2'):
             for bi in range(2):
                 p = f'head.{layer}.{bi}'
@@ -159,7 +146,6 @@ class CAMPPlus(Backbone):
                 bias=o['head.c2']['b'], act=L.ACT_RELU)
         pb.free(x)
         # ---- [B, T, F8, 32] viewed as [B*T, F8*32]; TDNN layer k5 stride 2 ----
-        from ..engine import View
         flat = View(y.off, fo * m, 0, fo * m)
         T2 = out_len(T, 5, 2, 2)
         ch = self.init_channels
@@ -202,9 +188,3 @@ class CAMPPlus(Backbone):
         pb.free(cat)
         pb.conv(stats, pb.output_view(self.embd_dim, B), o['dense']['w'], 2 * ch, 1, 1, bias=o['dense']['b'],
                 engine=L.ENGINE_FFMA)
-
-
-def L_view1(v):
-    """The [B*T, F] feature matrix seen as a one-channel [B, T, F, 1] map: row stride 1, one column."""
-    from ..engine import View
-    return View(v.off, 1, 0, 1)

@@ -4,6 +4,8 @@ conv2d W axis and F (frequency) the H axis of the reference's [B, C, F, T] tenso
 in (f, c) order instead of the reference's (c, f) -- the permutation is folded into the next layer's weights."""
 import numpy as np
 
+from .. import _lib as L
+from ..engine import View
 from .base import _np64, bn_affine
 
 
@@ -21,6 +23,12 @@ def fold_conv_bn(sd, conv_key, bn_prefix, bias_key=None):
     return W * s[:, None], b * s + h
 
 
+def pack_conv_bn(sd, arena, o, name, conv_key, bn_prefix):
+    """o[name] = the conv ``conv_key`` with its BN folded in, packed as dict(w=..., b=...)."""
+    W, b = fold_conv_bn(sd, conv_key, bn_prefix)
+    o[name] = dict(w=arena.add_conv(name + '.w', W), b=arena.add(name + '.b', b))
+
+
 def out_len(n, k, s, pad, dil=1):
     return (n + 2 * pad - dil * (k - 1) - 1) // s + 1
 
@@ -32,10 +40,19 @@ def fc_perm(F8, C):
     return (c * F8 + f).reshape(-1)
 
 
-def bn_names(d, p, c, affine=True):
-    if affine:
-        d[p + '.weight'] = (c,)
-        d[p + '.bias'] = (c,)
-    d[p + '.running_mean'] = (c,)
-    d[p + '.running_var'] = (c,)
-    d[p + '.num_batches_tracked'] = ()
+def L_view1(v):
+    """The [B*T, F] feature matrix seen as a one-channel [B, T, F, 1] map: row stride 1, one column."""
+    return View(v.off, 1, 0, 1)
+
+
+def lower_stem_c1(pb, e, B, T, F, C, k=3, stride=1, pad=1):
+    """The stem on the one-channel feature map: k x k stride-s conv2d (CONV_C1, BN folded in ``e``, ReLU) of the
+    [B*T, F] input into a [B, t, f, C] map.  Returns (map, t, f)."""
+    x_in = pb.input_view(F, B * T)
+    t, f = out_len(T, k, stride, pad), out_len(F, k, stride, pad)
+    if t < 1 or f < 1:
+        raise ValueError(f'{T} frames x {F} bins is too small for the {k}x{k} stride-{stride} stem')
+    x = pb.alloc(B * t * f, C)
+    pb.conv(L_view1(x_in), x, e['w'], k * k, T, t, Fin=F, Fout=f, KT=k, KF=k, sT=stride, sF=stride, padT=pad, padF=pad,
+            bias=e['b'], act=L.ACT_RELU, c1=True)
+    return x, t, f

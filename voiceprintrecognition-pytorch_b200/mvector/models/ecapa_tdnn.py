@@ -9,32 +9,15 @@ Lowering of one SERes2NetBlock (ecapa_tdnn.py:87-143), activations channel-last 
 """
 from collections import OrderedDict
 
-import os
-
-import numpy as np
-
 from .. import _lib as L
-from .base import Backbone, _np64, bn_affine
-from .pooling import check_pooling_type, lower_pool, pack_pool, pool_shapes, pool_width
+from .base import Backbone, _np64, bn_affine, bn_names, conv1d_weight
+from .pooling import check_pooling_type, head_shapes, lower_head, pack_head
 
 
 def _tdnn_block_shapes(d, p, cin, cout, k):
     d[p + '.conv.conv.weight'] = (cout, cin, k)
     d[p + '.conv.conv.bias'] = (cout,)
-    for n in ('weight', 'bias', 'running_mean', 'running_var'):
-        d[p + '.norm.norm.' + n] = (cout,)
-    d[p + '.norm.norm.num_batches_tracked'] = ()
-
-
-def conv1d_weight(w):
-    """[Cout, Cin, k] -> [Cout, k*Cin4] with K index = tap*Cin4 + ci (the gather order of the CONV op).  Cin4 = Cin
-    rounded up to a multiple of 4 with zero columns: only a first layer fed by an odd feature dim (Spectrogram's
-    n_fft/2+1 bins) is ever padded; its input comes through PlanBuilder.input_view1d."""
-    w = _np64(w)
-    cin = w.shape[1]
-    if cin % 4:
-        w = np.concatenate([w, np.zeros((w.shape[0], -cin % 4, w.shape[2]), dtype=w.dtype)], axis=1)
-    return np.ascontiguousarray(w.transpose(0, 2, 1)).reshape(w.shape[0], -1)
+    bn_names(d, p + '.norm.norm', cout)
 
 
 class EcapaTdnn(Backbone):
@@ -46,6 +29,7 @@ class EcapaTdnn(Backbone):
         assert len(channels) == len(kernel_sizes) and len(channels) == len(dilations)
         check_pooling_type(pooling_type)
         self.pooling_type = pooling_type
+        self.head_bn = 'asp_bn.norm' if pooling_type == 'ASP' else 'asp_bn'     # ecapa_tdnn.py:224 vs :232,239,246
         if activation is not None or not global_context or any(g != 1 for g in groups):
             raise NotImplementedError('EcapaTdnn: only ReLU / global_context=True / groups=1 are lowered')
         for c in channels[:-1]:
@@ -76,13 +60,8 @@ class EcapaTdnn(Backbone):
                 d[p + '.shortcut.conv.weight'] = (c, cin, 1)
                 d[p + '.shortcut.conv.bias'] = (c,)
         _tdnn_block_shapes(d, 'mfa', ch[-1], ch[-1], ks[-1])
-        width = pool_shapes(d, 'asp', self.pooling_type, ch[-1], self.attention_channels)
-        bn = 'asp_bn.norm' if self.pooling_type == 'ASP' else 'asp_bn'          # ecapa_tdnn.py:224 vs :232,239,246
-        for n in ('weight', 'bias', 'running_mean', 'running_var'):
-            d[f'{bn}.{n}'] = (width,)
-        d[bn + '.num_batches_tracked'] = ()
-        d['fc.conv.weight'] = (self.embd_dim, width, 1)
-        d['fc.conv.bias'] = (self.embd_dim,)
+        head_shapes(d, self.pooling_type, ch[-1], self.embd_dim, self.head_bn, 'fc.conv', pool='asp',
+                    att=self.attention_channels, fc_conv1d=True)
         return d
 
     # ---- weights ----
@@ -111,12 +90,7 @@ class EcapaTdnn(Backbone):
                 blk['sc_b'] = arena.add(p + '.sc.b', sd[p + '.shortcut.conv.bias'])
             o[p] = blk
         o['mfa'] = self._pack_tdnn_block(sd, 'mfa', arena)
-        o['asp'] = pack_pool(sd, 'asp', self.pooling_type, arena, ch[-1])
-        # asp_bn -> fc (ecapa_tdnn.py:278-281) is affine-then-linear: fold into one [embd, width] product (fp64 fold)
-        s, h = bn_affine(sd, 'asp_bn.norm' if self.pooling_type == 'ASP' else 'asp_bn')
-        W = _np64(sd['fc.conv.weight'])[:, :, 0]
-        o['fc_w'] = arena.add('fc.w', W * s[None, :])
-        o['fc_b'] = arena.add('fc.b', W @ h + _np64(sd['fc.conv.bias']))
+        o['head'] = pack_head(sd, arena, self.pooling_type, ch[-1], self.head_bn, 'fc.conv', pool='asp')
 
     # ---- program ----
     def _tdnn_block(self, pb, src, dst, w, T, k=1, dil=1, src2=None):
@@ -183,9 +157,4 @@ class EcapaTdnn(Backbone):
         self._tdnn_block(pb, cat, xm, o['mfa'], T, ks[-1], dl[-1])
         pb.free(cat)
         pb.tap('mfa', xm, M)
-        width = pool_width(self.pooling_type, ch[-1])
-        pooled = pb.alloc(B, width)
-        lower_pool(pb, o['asp'], self.pooling_type, xm, B, T, pooled)
-        pb.tap('pooled', pooled, B)
-        pb.conv(pooled, pb.output_view(self.embd_dim, B), o['fc_w'], width, 1, 1, bias=o['fc_b'],
-                engine=L.ENGINE_FFMA)
+        pb.tap('pooled', lower_head(pb, o['head'], self.pooling_type, xm, B, T, self.embd_dim), B)

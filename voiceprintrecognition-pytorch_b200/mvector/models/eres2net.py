@@ -22,9 +22,8 @@ import numpy as np
 
 from .. import _lib as L
 from ..engine import View
-from .base import Backbone, _np64
-from .campplus import L_view1
-from .conv2d_util import bn_names, conv2d_weight, fc_perm, fold_conv_bn, out_len
+from .base import Backbone, _np64, bn_names
+from .conv2d_util import conv2d_weight, fc_perm, fold_conv_bn, lower_stem_c1, out_len, pack_conv_bn
 
 HT = L.ACT_HARDTANH20
 
@@ -152,12 +151,7 @@ class ERes2Net(Backbone):
 
     def _pack(self, sd, arena):
         o, g = self._off, self.scale
-
-        def cb(name, conv_key, bn):
-            W, b = fold_conv_bn(sd, conv_key, bn)
-            o[name] = dict(w=arena.add_conv(name + '.w', W), b=arena.add(name + '.b', b))
-
-        cb('stem', 'conv1.weight', 'bn1')
+        pack_conv_bn(sd, arena, o, 'stem', 'conv1.weight', 'bn1')
         for p, li, inpl, planes, w, stride, fuse, sc in self._blocks():
             wp = _pad4(w)
             W, b = fold_conv_bn(sd, p + '.conv1.weight', p + '.bn1')                       # [g*w, inpl]
@@ -174,7 +168,7 @@ class ERes2Net(Backbone):
             W, b = fold_conv_bn(sd, p + '.conv3.weight', p + '.bn3')                       # [planes*exp, g*w]
             o[p + '.c3'] = dict(w=arena.add_conv(p + '.c3.w', _grp_cols(W, w, wp, g)), b=arena.add(p + '.c3.b', b))
             if sc:
-                cb(p + '.sc', p + '.shortcut.0.weight', p + '.shortcut.1')
+                pack_conv_bn(sd, arena, o, p + '.sc', p + '.shortcut.0.weight', p + '.shortcut.1')
         self._pack_top(sd, arena)
         C4 = self.m * 8 * self.expansion
         perm = fc_perm(self.F8, C4)
@@ -219,12 +213,7 @@ class ERes2Net(Backbone):
 
     def _lower(self, pb, B, T):
         o, g = self._off, self.scale
-        F = self.input_size
-        x_in = pb.input_view(F, B * T)
-        x = pb.alloc(B * T * F, self.m)
-        pb.conv(L_view1(x_in), x, o['stem']['w'], 9, T, T, Fin=F, Fout=F, KT=3, KF=3, padT=1, padF=1,
-                bias=o['stem']['b'], act=L.ACT_RELU, c1=True)
-        t, f = T, F
+        x, t, f = lower_stem_c1(pb, o['stem'], B, T, self.input_size, self.m)
         layer_out = {}
         last_li = 1
         for p, li, inpl, planes, w, stride, fuse, sc in self._blocks():

@@ -12,15 +12,13 @@ second term is a per-utterance bias computed once by a [B, 2C] x [2C, A] product
 import numpy as np
 
 from .. import _lib as L
-from .base import _np64, bn_affine
+from .base import _np64, bn_affine, bn_names
 
 
 def asp_shapes(d, p, c, att=128):
     d[p + '.tdnn.conv.conv.weight'] = (att, c * 3, 1)
     d[p + '.tdnn.conv.conv.bias'] = (att,)
-    for n in ('weight', 'bias', 'running_mean', 'running_var'):
-        d[p + '.tdnn.norm.norm.' + n] = (att,)
-    d[p + '.tdnn.norm.norm.num_batches_tracked'] = ()
+    bn_names(d, p + '.tdnn.norm.norm', att)
     d[p + '.conv.conv.weight'] = (c, att, 1)
     d[p + '.conv.conv.bias'] = (c,)
 
@@ -126,3 +124,45 @@ def lower_pool(pb, o, kind, x, B, T, pooled):
         pb.asp_pool(x, logits, pooled, T, mean_only=True)
         pb.free(logits)
         pb.free(h)
+
+
+# ---------------------------------------------------------------------------------------------------------------
+# The embedding head shared by ECAPA, TDNN, ResNetSE and Res2Net: pooling -> BN `bn` -> linear `fc` (-> BN `post_bn`).
+# The BN(s) and the linear layer are affine, so they collapse into one [embd, width] product folded in fp64 at pack time.
+# ---------------------------------------------------------------------------------------------------------------
+def head_shapes(d, kind, c, embd, bn, fc, post_bn=None, pool='pooling', att=128, fc_conv1d=False):
+    """``fc_conv1d``: the linear layer is a kernel-1 Conv1d (weight [embd, width, 1]) instead of an nn.Linear."""
+    width = pool_shapes(d, pool, kind, c, att)
+    bn_names(d, bn, width)
+    d[fc + '.weight'] = (embd, width, 1) if fc_conv1d else (embd, width)
+    d[fc + '.bias'] = (embd,)
+    if post_bn is not None:
+        bn_names(d, post_bn, embd)
+
+
+def pack_head(sd, arena, kind, c, bn, fc, post_bn=None, pool='pooling', perm=None):
+    """perm: the (f, c) column order of a 2-D backbone's flattened map (conv2d_util.fc_perm), folded into the weights."""
+    o = dict(pool=pack_pool(sd, pool, kind, arena, c, perm=perm))
+    s, h = bn_affine(sd, bn)
+    W = _np64(sd[fc + '.weight'])
+    W = W.reshape(W.shape[0], -1)
+    b = W @ h + _np64(sd[fc + '.bias'])
+    if post_bn is None:             # not an identity post-BN: multiplying by s2 = 1 can still change a -0 into +0
+        W = W * s[None, :]
+    else:
+        s2, h2 = bn_affine(sd, post_bn)
+        W, b = s2[:, None] * W * s[None, :], s2 * b + h2
+    if perm is not None:
+        W = W[:, pool_perm(kind, c, perm)]
+    o['w'], o['b'] = arena.add('fc.w', W), arena.add('fc.b', b)
+    return o
+
+
+def lower_head(pb, o, kind, x, B, T, embd):
+    """x: View [B*T, C], freed after pooling.  Writes the embeddings [B, embd] and returns the pooled View [B, width]."""
+    width = pool_width(kind, x.C)
+    pooled = pb.alloc(B, width)
+    lower_pool(pb, o['pool'], kind, x, B, T, pooled)
+    pb.free(x)
+    pb.conv(pooled, pb.output_view(embd, B), o['w'], width, 1, 1, bias=o['b'], engine=L.ENGINE_FFMA)
+    return pooled

@@ -12,14 +12,11 @@
 import math
 from collections import OrderedDict
 
-import numpy as np
-
 from .. import _lib as L
 from ..engine import View
-from .base import Backbone, _np64, bn_affine
-from .campplus import L_view1
-from .conv2d_util import bn_names, fc_perm, fold_conv_bn, out_len
-from .pooling import check_pooling_type, lower_pool, pack_pool, pool_perm, pool_shapes, pool_width
+from .base import Backbone, bn_names
+from .conv2d_util import fc_perm, lower_stem_c1, out_len, pack_conv_bn
+from .pooling import check_pooling_type, head_shapes, lower_head, pack_head
 
 
 class Res2Net(Backbone):
@@ -63,49 +60,27 @@ class Res2Net(Backbone):
             if ds:
                 d[p + '.downsample.0.weight'] = (planes * 4, inpl, 1, 1)
                 bn_names(d, p + '.downsample.1', planes * 4)
-        width = pool_shapes(d, 'pooling', self.pooling_type, self.cat, 128)
-        bn_names(d, 'bn2', width)
-        d['linear.weight'] = (self.embd_dim, width)
-        d['linear.bias'] = (self.embd_dim,)
-        bn_names(d, 'bn3', self.embd_dim)
+        head_shapes(d, self.pooling_type, self.cat, self.embd_dim, 'bn2', 'linear', 'bn3')
         return d
 
     def _pack(self, sd, arena):
         o = self._off
-
-        def cb(name, conv_key, bn):
-            W, b = fold_conv_bn(sd, conv_key, bn)
-            o[name] = dict(w=arena.add_conv(name + '.w', W), b=arena.add(name + '.b', b))
-
-        cb('stem', 'conv1.weight', 'bn1')
+        pack_conv_bn(sd, arena, o, 'stem', 'conv1.weight', 'bn1')
         for p, inpl, planes, w, stride, stage, ds in self._blocks():
-            cb(p + '.c1', p + '.conv1.weight', p + '.bn1')
+            pack_conv_bn(sd, arena, o, p + '.c1', p + '.conv1.weight', p + '.bn1')
             for j in range(self.scale - 1):
-                cb(f'{p}.k{j}', f'{p}.convs.{j}.weight', f'{p}.bns.{j}')
-            cb(p + '.c3', p + '.conv3.weight', p + '.bn3')
+                pack_conv_bn(sd, arena, o, f'{p}.k{j}', f'{p}.convs.{j}.weight', f'{p}.bns.{j}')
+            pack_conv_bn(sd, arena, o, p + '.c3', p + '.conv3.weight', p + '.bn3')
             if ds:
-                cb(p + '.ds', p + '.downsample.0.weight', p + '.downsample.1')
+                pack_conv_bn(sd, arena, o, p + '.ds', p + '.downsample.0.weight', p + '.downsample.1')
         C4 = self.m * 8 * 4
-        f_last = self.cat // C4
-        perm = fc_perm(f_last, C4)
-        o['pool'] = pack_pool(sd, 'pooling', self.pooling_type, arena, self.cat, perm=perm)
-        s2, h2 = bn_affine(sd, 'bn2')
-        s3, h3 = bn_affine(sd, 'bn3')
-        W, b = _np64(sd['linear.weight']), _np64(sd['linear.bias'])
-        Wf = s3[:, None] * W * s2[None, :]
-        o['fc_w'] = arena.add('fc.w', Wf[:, pool_perm(self.pooling_type, self.cat, perm)])
-        o['fc_b'] = arena.add('fc.b', s3 * (W @ h2 + b) + h3)
+        o['head'] = pack_head(sd, arena, self.pooling_type, self.cat, 'bn2', 'linear', 'bn3',
+                              perm=fc_perm(self.cat // C4, C4))
 
     def _lower(self, pb, B, T):
         o, sc = self._off, self.scale
         F = self.input_size
-        x_in = pb.input_view(F, B * T)
-        t, f = out_len(T, 7, 3, 1), out_len(F, 7, 3, 1)
-        if t < 1 or f < 1:
-            raise ValueError(f'{T} frames x {F} bins is too small for the 7x7 stride-3 stem')
-        s0 = pb.alloc(B * t * f, self.m)
-        pb.conv(L_view1(x_in), s0, o['stem']['w'], 49, T, t, Fin=F, Fout=f, KT=7, KF=7, sT=3, sF=3, padT=1, padF=1,
-                bias=o['stem']['b'], act=L.ACT_RELU, c1=True)
+        s0, t, f = lower_stem_c1(pb, o['stem'], B, T, F, self.m, k=7, stride=3)
         tp, fp = out_len(t, 3, 2, 1), out_len(f, 3, 2, 1)
         x = pb.alloc(B * tp * fp, self.m)
         pb.pool2d(s0, x, L.POOL_MAX, t, f, tp, fp, k=3, stride=2, pad=1)
@@ -148,9 +123,4 @@ class Res2Net(Backbone):
         if f * C4 != self.cat:
             raise ValueError(f'input_size {F}: the flattened map has {f * C4} channels but the head was built for '
                              f'{self.cat} = m_channels*32*(input_size // base_width) (res2net.py:111)')
-        flat = View(x.off, f * C4, 0, f * C4)
-        width = pool_width(self.pooling_type, self.cat)
-        pooled = pb.alloc(B, width)
-        lower_pool(pb, o['pool'], self.pooling_type, flat, B, t, pooled)
-        pb.free(x)
-        pb.conv(pooled, pb.output_view(self.embd_dim, B), o['fc_w'], width, 1, 1, bias=o['fc_b'], engine=L.ENGINE_FFMA)
+        lower_head(pb, o['head'], self.pooling_type, View(x.off, f * C4, 0, f * C4), B, t, self.embd_dim)

@@ -7,14 +7,11 @@ The final reshape to [B, C*F/8, T/8] is free in this layout; ASP / bn2 / linear 
 bn2 -> linear -> bn3 collapse into one product."""
 from collections import OrderedDict
 
-import numpy as np
-
 from .. import _lib as L
 from ..engine import View
-from .base import Backbone, _np64, bn_affine
-from .campplus import L_view1
-from .conv2d_util import bn_names, fc_perm, fold_conv_bn, out_len
-from .pooling import check_pooling_type, lower_pool, pack_pool, pool_perm, pool_shapes, pool_width
+from .base import Backbone, bn_names
+from .conv2d_util import fc_perm, lower_stem_c1, out_len, pack_conv_bn
+from .pooling import check_pooling_type, head_shapes, lower_head, pack_head
 
 
 class ResNetSE(Backbone):
@@ -55,51 +52,28 @@ class ResNetSE(Backbone):
             if ds:
                 d[p + '.downsample.0.weight'] = (planes * 2, inpl, 1, 1)
                 bn_names(d, p + '.downsample.1', planes * 2)
-        width = pool_shapes(d, 'pooling', self.pooling_type, self.cat, 128)
-        bn_names(d, 'bn2', width)
-        d['linear.weight'] = (self.embd_dim, width)
-        d['linear.bias'] = (self.embd_dim,)
-        bn_names(d, 'bn3', self.embd_dim)
+        head_shapes(d, self.pooling_type, self.cat, self.embd_dim, 'bn2', 'linear', 'bn3')
         return d
 
     def _pack(self, sd, arena):
         o = self._off
-
-        def cb(name, conv_key, bn):
-            W, b = fold_conv_bn(sd, conv_key, bn)
-            o[name] = dict(w=arena.add_conv(name + '.w', W), b=arena.add(name + '.b', b))
-
-        cb('stem', 'conv1.weight', 'bn1')
+        pack_conv_bn(sd, arena, o, 'stem', 'conv1.weight', 'bn1')
         for p, inpl, planes, stride, ds in self._blocks():
-            cb(p + '.c1', p + '.conv1.weight', p + '.bn1')
-            cb(p + '.c2', p + '.conv2.weight', p + '.bn2')
-            cb(p + '.c3', p + '.conv3.weight', p + '.bn3')
+            pack_conv_bn(sd, arena, o, p + '.c1', p + '.conv1.weight', p + '.bn1')
+            pack_conv_bn(sd, arena, o, p + '.c2', p + '.conv2.weight', p + '.bn2')
+            pack_conv_bn(sd, arena, o, p + '.c3', p + '.conv3.weight', p + '.bn3')
             if ds:
-                cb(p + '.ds', p + '.downsample.0.weight', p + '.downsample.1')
+                pack_conv_bn(sd, arena, o, p + '.ds', p + '.downsample.0.weight', p + '.downsample.1')
             o[p + '.se'] = dict(w1=arena.add(p + '.se.w1', sd[p + '.se.fc.0.weight']),
                                 b1=arena.add(p + '.se.b1', sd[p + '.se.fc.0.bias']),
                                 w2=arena.add(p + '.se.w2', sd[p + '.se.fc.2.weight']),
                                 b2=arena.add(p + '.se.b2', sd[p + '.se.fc.2.bias']))
-        C4 = self.nf[3] * 2
-        perm = fc_perm(self.F8, C4)
-        o['asp'] = pack_pool(sd, 'pooling', self.pooling_type, arena, self.cat, perm=perm)
-        s2, h2 = bn_affine(sd, 'bn2')
-        s3, h3 = bn_affine(sd, 'bn3')
-        W, b = _np64(sd['linear.weight']), _np64(sd['linear.bias'])
-        Wf = s3[:, None] * W * s2[None, :]
-        bf = s3 * (W @ h2 + b) + h3
-        o['fc_w'] = arena.add('fc.w', Wf[:, pool_perm(self.pooling_type, self.cat, perm)])
-        o['fc_b'] = arena.add('fc.b', bf)
+        o['head'] = pack_head(sd, arena, self.pooling_type, self.cat, 'bn2', 'linear', 'bn3',
+                              perm=fc_perm(self.F8, self.nf[3] * 2))
 
     def _lower(self, pb, B, T):
         o = self._off
-        F = self.input_size
-        x_in = pb.input_view(F, B * T)
-        c = self.nf[0]
-        x = pb.alloc(B * T * F, c)
-        pb.conv(L_view1(x_in), x, o['stem']['w'], 9, T, T, Fin=F, Fout=F, KT=3, KF=3, padT=1, padF=1,
-                bias=o['stem']['b'], act=L.ACT_RELU, c1=True)
-        t, f = T, F
+        x, t, f = lower_stem_c1(pb, o['stem'], B, T, self.input_size, self.nf[0])
         for p, inpl, planes, stride, ds in self._blocks():
             to, fo = out_len(t, 3, stride, 1), out_len(f, 3, stride, 1)
             h1 = pb.alloc(B * t * f, planes)
@@ -133,10 +107,4 @@ class ResNetSE(Backbone):
             x, t, f = y, to, fo
         assert f == self.F8, 'input_size must be a multiple of 8'
         C4 = self.nf[3] * 2
-        flat = View(x.off, f * C4, 0, f * C4)
-        width = pool_width(self.pooling_type, self.cat)
-        pooled = pb.alloc(B, width)
-        lower_pool(pb, o['asp'], self.pooling_type, flat, B, t, pooled)
-        pb.free(x)
-        pb.conv(pooled, pb.output_view(self.embd_dim, B), o['fc_w'], width, 1, 1, bias=o['fc_b'],
-                engine=L.ENGINE_FFMA)
+        lower_head(pb, o['head'], self.pooling_type, View(x.off, f * C4, 0, f * C4), B, t, self.embd_dim)

@@ -2,12 +2,9 @@
 relu(conv) -> BN (tdnn.py:57-65; the 5th has no BN), ASP(512), bn5 -> linear -> bn6 folded into one product."""
 from collections import OrderedDict
 
-import numpy as np
-
 from .. import _lib as L
-from .base import Backbone, _np64, bn_affine
-from .ecapa_tdnn import conv1d_weight
-from .pooling import check_pooling_type, lower_pool, pack_pool, pool_shapes, pool_width
+from .base import Backbone, bn_affine, bn_names, conv1d_weight
+from .pooling import check_pooling_type, head_shapes, lower_head, pack_head
 
 _KS = (5, 3, 3, 1, 1)
 _DIL = (1, 2, 3, 1, 1)
@@ -27,19 +24,8 @@ class TDNN(Backbone):
             d[f'td_layer{i}.weight'] = (c, self.input_size if i == 1 else c, k)
             d[f'td_layer{i}.bias'] = (c,)
             if i < 5:
-                for n in ('weight', 'bias', 'running_mean', 'running_var'):
-                    d[f'bn{i}.{n}'] = (c,)
-                d[f'bn{i}.num_batches_tracked'] = ()
-        width = pool_shapes(d, 'pooling', self.pooling_type, c, 128)
-        for nm, n_ in (('bn5', width),):
-            for n in ('weight', 'bias', 'running_mean', 'running_var'):
-                d[f'{nm}.{n}'] = (n_,)
-            d[f'{nm}.num_batches_tracked'] = ()
-        d['linear.weight'] = (self.embd_dim, width)
-        d['linear.bias'] = (self.embd_dim,)
-        for n in ('weight', 'bias', 'running_mean', 'running_var'):
-            d[f'bn6.{n}'] = (self.embd_dim,)
-        d['bn6.num_batches_tracked'] = ()
+                bn_names(d, f'bn{i}', c)
+        head_shapes(d, self.pooling_type, c, self.embd_dim, 'bn5', 'linear', 'bn6')
         return d
 
     def _pack(self, sd, arena):
@@ -51,12 +37,7 @@ class TDNN(Backbone):
                 s, h = bn_affine(sd, f'bn{i}')
                 e['s'], e['h'] = arena.add(f'bn{i}.s', s), arena.add(f'bn{i}.h', h)
             o[f'td{i}'] = e
-        o['asp'] = pack_pool(sd, 'pooling', self.pooling_type, arena, self.channels)
-        s5, h5 = bn_affine(sd, 'bn5')
-        s6, h6 = bn_affine(sd, 'bn6')
-        W, b = _np64(sd['linear.weight']), _np64(sd['linear.bias'])
-        o['fc_w'] = arena.add('fc.w', s6[:, None] * W * s5[None, :])
-        o['fc_b'] = arena.add('fc.b', s6 * (W @ h5 + b) + h6)
+        o['head'] = pack_head(sd, arena, self.pooling_type, self.channels, 'bn5', 'linear', 'bn6')
 
     def _lower(self, pb, B, T):
         o, c = self._off, self.channels
@@ -73,8 +54,4 @@ class TDNN(Backbone):
             if x.off != L.BUF_INPUT:
                 pb.free(x)
             x, t = y, tout
-        width = pool_width(self.pooling_type, c)
-        pooled = pb.alloc(B, width)
-        lower_pool(pb, o['asp'], self.pooling_type, x, B, t, pooled)
-        pb.free(x)
-        pb.conv(pooled, pb.output_view(self.embd_dim, B), o['fc_w'], width, 1, 1, bias=o['fc_b'], engine=L.ENGINE_FFMA)
+        lower_head(pb, o['head'], self.pooling_type, x, B, t, self.embd_dim)
