@@ -43,18 +43,20 @@ typedef struct vp_handle vp_handle;
 typedef struct vp_program vp_program;
 
 /* ------------------------------------------------------------------------------------------------------------
- * Front-end (seam 1).  kind 0 = Kaldi Fbank framing (snip_edges, per-frame DC removal, pre-emphasis, window,
- * zero-pad to n_fft; kaldi.py:154-217), kind 1 = torch.stft framing (reflect-centred frames of n_fft samples,
- * functional.py:123-135).  Then |rFFT|^2 (power 2) or |rFFT| (power 1), sparse triangular mel projection,
- * optional log(max(x, log_floor)), then (featurizer.py:77-90) time-mean subtraction over ALL T frames and zeroing
- * of frames >= keep_frames[b].
+ * Front-end (seam 1).  kind 0 = Kaldi Fbank framing (per-frame DC removal, pre-emphasis, window, zero-pad to n_fft;
+ * kaldi.py:154-217), kind 1 = torch.stft framing (frames of n_fft samples, functional.py:123-135).  Which samples a
+ * frame takes (snip_edges or reflected edges; centred in one of four pad modes or not centred, after `pad` zeros) is
+ * set by vp_frontend_set_options; vp_frontend_set selects the default framing of the kind.  Then |rFFT|^2 (power 2)
+ * or |rFFT| (power 1), optionally scaled first (`normalized`), sparse triangular mel projection, optional
+ * log(max(x, log_floor)), then (featurizer.py:77-90) time-mean subtraction over ALL T frames and zeroing of frames
+ * >= keep_frames[b].
  * ---------------------------------------------------------------------------------------------------------- */
 typedef struct vp_frontend_desc {
   int32_t kind;         /* 0 kaldi-fbank framing, 1 centred-STFT framing */
-  int32_t n_fft;        /* FFT size N = 2^a 3^b 5^c, multiple of 4, in [64, 2048]; kind 0 needs a power of two */
+  int32_t n_fft;        /* FFT size N = 2^a 3^b 5^c, multiple of 4, in [64, 2048] */
   int32_t win_length;   /* samples taken per frame (<= n_fft); window[] has this many taps */
   int32_t hop;          /* frame shift in samples */
-  int32_t n_mels;       /* filter count: <= 128 mel filters, or n_fft/2+1 (<= 1025) pass-through bins for Spectrogram */
+  int32_t n_mels;       /* filter count, <= n_fft/2+1 (<= 1025): mel filters (<= 128 for MFCC) or Spectrogram bins */
   int32_t remove_dc;    /* kind 0: subtract the frame mean */
   float   preemph;      /* kind 0: pre-emphasis coefficient (0 = off) */
   int32_t power;        /* 2 = power spectrum, 1 = magnitude */
@@ -78,9 +80,32 @@ int32_t vp_sizeof_frontend_desc(void);  /* binding self-check: sizeof(vp_fronten
  * (torchaudio create_dct layout) when desc->post == 1, else NULL; all host pointers, copied. */
 int vp_frontend_set(vp_handle* h, const vp_frontend_desc* desc, const float* window, const int32_t* mel_start,
                     const int32_t* mel_count, const int32_t* mel_off, const float* mel_w, int32_t n_w, const float* dct);
+
+/* Framing and spectrum scale of the configured front-end.  vp_frontend_set resets them to the defaults
+ * {VP_FRAME_DEFAULT, 0, 1.0}, which give kind 0 snip_edges framing and kind 1 centred reflect framing.  With L' = L + 2 pad:
+ *   VP_FRAME_DEFAULT, kind 0   frames [t hop, t hop + win_length), T = 1 + (L - win_length) / hop       (snip_edges)
+ *   VP_FRAME_KALDI_REFLECT     kind 0: T = (L + hop/2) / hop frames of the signal extended half-sample-symmetrically at
+ *                              both ends, starting win_length/2 - hop/2 samples before x[0] (kaldi.py:44-83)
+ *   VP_FRAME_DEFAULT, kind 1   T = 1 + L' / hop frames centred on t hop, the n_fft/2 samples beyond each end of the
+ *                              zero-extended signal reflected (torch.stft center=True, pad_mode 'reflect')
+ *   VP_FRAME_STFT_CONSTANT / _REPLICATE / _CIRCULAR   kind 1: the same with zeros, the edge sample, or wrap-around
+ *   VP_FRAME_STFT_NOCENTER     kind 1: T = 1 + (L' - n_fft) / hop frames, no centring (center=False)
+ * Each call fails with VP_ERR_INVALID before any launch when the waveform length breaks what torch requires:
+ * kind 0: 2 <= win_length <= L; reflect: n_fft/2 < L'; circular: n_fft/2 <= L'; not centred: n_fft <= L'. */
+enum { VP_FRAME_DEFAULT = 0, VP_FRAME_KALDI_REFLECT = 1, VP_FRAME_STFT_CONSTANT = 2, VP_FRAME_STFT_REPLICATE = 3,
+       VP_FRAME_STFT_CIRCULAR = 4, VP_FRAME_STFT_NOCENTER = 5 };
+typedef struct vp_frontend_options {
+  int32_t frame_mode;   /* VP_FRAME_*: must fit the configured kind */
+  int32_t pad;          /* kind 1: zeros added at both ends before framing (torchaudio `pad`); 0 for kind 0 */
+  double  spec_scale;   /* kind 1: |X| multiplier before |.|^power (1/sqrt(sum w^2) or 1/sqrt(n_fft): `normalized`);
+                           1.0 = none, the only value for kind 0 */
+} vp_frontend_options;
+int vp_frontend_set_options(vp_handle* h, const vp_frontend_options* opts);   /* after vp_frontend_set */
+int32_t vp_sizeof_frontend_options(void);  /* binding self-check: sizeof(vp_frontend_options) */
+
 /* feature dimension F the configured front-end emits (n_mels, or n_out for MFCC) */
 int32_t vp_feature_dim(const vp_handle* h);
-/* number of frames T the configured front-end yields for n_samples (kaldi.py:63-67 / torch.stft) */
+/* number of frames T the configured front-end yields for n_samples (kaldi.py:63-83 / torch.stft; see the framing above) */
 int32_t vp_num_frames(const vp_handle* h, int32_t n_samples);
 
 /* wave [B, Lpad] (zero padded to the batch max, predict.py:248-254) -> feats [B, T, F], T = vp_num_frames(Lpad).

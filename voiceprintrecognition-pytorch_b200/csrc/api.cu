@@ -27,6 +27,7 @@ struct vp_handle {
   // front-end
   bool fe_set = false;
   vp_frontend_desc fe{};
+  vp_frontend_options fe_opt{VP_FRAME_DEFAULT, 0, 1.0};
   float* d_window = nullptr;
   double2* d_twiddle = nullptr;
   int* d_mel_start = nullptr;
@@ -87,6 +88,7 @@ static void fill_conv(const vp_program* p, const vp_op& o, const float* feats, f
 int vp_abi_version(void) { return VP_ABI_VERSION; }
 int32_t vp_sizeof_op(void) { return (int32_t)sizeof(vp_op); }
 int32_t vp_sizeof_frontend_desc(void) { return (int32_t)sizeof(vp_frontend_desc); }
+int32_t vp_sizeof_frontend_options(void) { return (int32_t)sizeof(vp_frontend_options); }
 
 int vp_create(int device, vp_handle** out) {
   if (!out) return VP_ERR_INVALID;
@@ -135,7 +137,6 @@ int vp_frontend_set(vp_handle* h, const vp_frontend_desc* d, const float* window
   if (N < 64 || N > 2048 || (N & 3) || rem != 1)
     return fail(h, VP_ERR_UNSUPPORTED, "n_fft %d: need 2^a 3^b 5^c, a multiple of 4, in [64, 2048]", N);
   if (d->kind != 0 && d->kind != 1) return fail(h, VP_ERR_INVALID, "front-end kind %d", d->kind);
-  if (d->kind == 0 && (N & (N - 1))) return fail(h, VP_ERR_UNSUPPORTED, "kaldi framing needs a power-of-two n_fft");
   if (d->win_length < 2 || d->win_length > N || d->hop < 1) return fail(h, VP_ERR_INVALID, "bad window/hop");
   if (d->kind == 1 && d->win_length != N) return fail(h, VP_ERR_INVALID, "stft framing needs a window of n_fft taps");
   if (d->n_mels < 1 || d->n_mels > N / 2 + 1) return fail(h, VP_ERR_UNSUPPORTED, "n_mels %d out of range", d->n_mels);
@@ -178,14 +179,48 @@ int vp_frontend_set(vp_handle* h, const vp_frontend_desc* d, const float* window
     CUDA_TRY(h, cudaMemcpy(h->d_dct, dct, sizeof(float) * F * d->n_out, cudaMemcpyHostToDevice));
   }
   h->fe = *d;
+  h->fe_opt = vp_frontend_options{VP_FRAME_DEFAULT, 0, 1.0};
   h->fe_set = true;
+  return VP_OK;
+}
+
+int vp_frontend_set_options(vp_handle* h, const vp_frontend_options* o) {
+  if (!h || !o) return fail(h, VP_ERR_INVALID, "null argument");
+  if (!h->fe_set) return fail(h, VP_ERR_INVALID, "front-end not configured (vp_frontend_set)");
+  const bool kaldi = h->fe.kind == 0;
+  const int m = o->frame_mode;
+  if (kaldi ? (m != VP_FRAME_DEFAULT && m != VP_FRAME_KALDI_REFLECT)
+            : (m != VP_FRAME_DEFAULT && (m < VP_FRAME_STFT_CONSTANT || m > VP_FRAME_STFT_NOCENTER)))
+    return fail(h, VP_ERR_INVALID, "frame mode %d does not fit front-end kind %d", m, h->fe.kind);
+  if (o->pad < 0 || (kaldi && o->pad != 0)) return fail(h, VP_ERR_INVALID, "pad %d (kind 1 only, >= 0)", o->pad);
+  if (!(o->spec_scale > 0.0) || !std::isfinite(o->spec_scale) || (kaldi && o->spec_scale != 1.0))
+    return fail(h, VP_ERR_INVALID, "spec_scale %g (finite, > 0; 1 for kind 0)", o->spec_scale);
+  h->fe_opt = *o;
   return VP_OK;
 }
 
 int32_t vp_num_frames(const vp_handle* h, int32_t n) {
   if (!h || !h->fe_set) return -1;
-  if (h->fe.kind == 0) return n < h->fe.win_length ? 0 : 1 + (n - h->fe.win_length) / h->fe.hop;
-  return 1 + n / h->fe.hop;
+  const int hop = h->fe.hop, mode = h->fe_opt.frame_mode;
+  if (h->fe.kind == 0) {
+    if (mode == VP_FRAME_KALDI_REFLECT) return (n + hop / 2) / hop;
+    return n < h->fe.win_length ? 0 : 1 + (n - h->fe.win_length) / hop;
+  }
+  const int64_t Lp = (int64_t)n + 2 * (int64_t)h->fe_opt.pad;
+  if (mode == VP_FRAME_STFT_NOCENTER) return Lp < h->fe.n_fft ? 0 : (int32_t)(1 + (Lp - h->fe.n_fft) / hop);
+  return (int32_t)(1 + Lp / hop);
+}
+
+// The waveform lengths torch accepts for the configured framing (kaldi.py:141, torch.stft / F.pad): "" when L fits.
+static const char* frontend_length_error(const vp_handle* h, int L) {
+  const int64_t Lp = (int64_t)L + 2 * (int64_t)h->fe_opt.pad, half = h->fe.n_fft / 2;
+  switch (h->fe.kind == 0 ? -1 : h->fe_opt.frame_mode) {
+    case -1: return (h->fe.win_length >= 2 && h->fe.win_length <= L) ? "" : "kaldi framing needs 2 <= win_length <= L";
+    case VP_FRAME_DEFAULT: return half < Lp ? "" : "reflect padding needs n_fft/2 < L + 2 pad";
+    case VP_FRAME_STFT_CIRCULAR: return half <= Lp ? "" : "circular padding needs n_fft/2 <= L + 2 pad";
+    case VP_FRAME_STFT_NOCENTER: return h->fe.n_fft <= Lp ? "" : "center=False needs n_fft <= L + 2 pad";
+    default: return L >= 1 ? "" : "empty waveform";
+  }
 }
 
 int32_t vp_feature_dim(const vp_handle* h) {
@@ -216,9 +251,10 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
   if (want_post >= 0 && h->fe.post != want_post) return fail(h, VP_ERR_INVALID, "front-end post-stage mismatch (vp_melspec vs vp_mfcc)");
   if ((stage != 2 && !wave) || (stage != 1 && !feats) || !scratch || B < 1) return fail(h, VP_ERR_INVALID, "null/empty argument");
   if (stage != 0 && (h->fe.post != 1 || !ext_max)) return fail(h, VP_ERR_INVALID, "two-stage calls are for the MFCC front-end");
+  const char* len_err = frontend_length_error(h, L);
+  if (*len_err) return fail(h, VP_ERR_INVALID, "waveform of %d samples: %s", L, len_err);
   const int T = vp_num_frames(h, L);
   if (T < 1) return fail(h, VP_ERR_INVALID, "waveform of %d samples is shorter than one frame (%d)", L, h->fe.win_length);
-  if (h->fe.kind == 1 && L <= h->fe.n_fft / 2) return fail(h, VP_ERR_INVALID, "reflect padding needs L > n_fft/2");
   CUDA_TRY(h, cudaSetDevice(h->device));
   FrontendParams p;
   p.wave = wave; p.feats = feats; p.partial = scratch;
@@ -227,6 +263,9 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
   p.B = B; p.L = L; p.T = T; p.kind = h->fe.kind; p.N = h->fe.n_fft; p.WL = h->fe.win_length; p.hop = h->fe.hop;
   p.F = h->fe.n_mels; p.remove_dc = h->fe.remove_dc; p.power = h->fe.power; p.use_log = h->fe.use_log;
   p.fpb = FPB; p.nblk = (T + FPB - 1) / FPB;
+  p.frame = h->fe_opt.frame_mode;
+  p.pad = p.kind == 0 ? p.WL / 2 - p.hop / 2 : h->fe_opt.pad;
+  p.spec_mult = h->fe.power == 2 ? h->fe_opt.spec_scale * h->fe_opt.spec_scale : h->fe_opt.spec_scale;
   p.preemph = h->fe.preemph; p.log_floor = h->fe.log_floor; p.db_mult = h->fe.db_mult; p.cta_max = nullptr;
   frontend_plan(p);
   if (h->fe.post == 1) {

@@ -65,20 +65,29 @@ __global__ void __launch_bounds__(256) frontend_kernel(const __grid_constant__ F
   float vmax = -INFINITY;
   const float* wv = p.wave + (size_t)b * p.L;
 
-  // ---- stage the waveform span, window and twiddles ----
+  // ---- stage the waveform span, window and twiddles; the frame mode maps each staged sample to its source ----
   const int q0 = f0 * p.hop;
   for (int i = tid; i < span; i += 256) {
     int s = q0 + i;
-    float v = 0.f;
-    if (p.kind == 1) {                      // torch.stft(center=True, pad_mode='reflect'): functional.py:123-135
-      s -= N / 2;
-      if (s < 0) s = -s;
-      if (s >= p.L) s = 2 * (p.L - 1) - s;
-      if (s >= 0 && s < p.L) v = __ldg(wv + s);
-    } else if (s < p.L) {
-      v = __ldg(wv + s);
+    if (p.kind == 1) {                      // torch.stft of x zero-extended by p.pad at both ends: functional.py:112-134
+      const int Lp = p.L + 2 * p.pad;
+      if (p.frame != VP_FRAME_STFT_NOCENTER) s -= N / 2;
+      if (p.frame == VP_FRAME_DEFAULT) {                  // reflect
+        if (s < 0) s = -s;
+        if (s >= Lp) s = 2 * (Lp - 1) - s;
+      } else if (p.frame == VP_FRAME_STFT_REPLICATE) {
+        s = min(max(s, 0), Lp - 1);
+      } else if (p.frame == VP_FRAME_STFT_CIRCULAR) {
+        if (s < 0) s += Lp;
+        if (s >= Lp) s -= Lp;
+      }                                                   // constant / not centred: outside is zero
+      s -= p.pad;
+    } else if (p.frame == VP_FRAME_KALDI_REFLECT) {       // kaldi._get_strided(snip_edges=False): x[-1-j] / x[2L-1-j]
+      s -= p.pad;
+      if (s < 0) s = -1 - s;
+      if (s >= p.L) s = 2 * p.L - 1 - s;
     }
-    stage[i] = v;
+    stage[i] = (s >= 0 && s < p.L) ? __ldg(wv + s) : 0.f;
   }
   for (int i = tid; i < WL; i += 256) win[i] = __ldg(p.window + i);
   for (int i = tid; i < N; i += 256) tw[i] = __ldg(p.twiddle + i);
@@ -231,6 +240,7 @@ __global__ void __launch_bounds__(256) frontend_kernel(const __grid_constant__ F
       const double br = 0.5 * (z.y + zn.y), bi = -0.5 * (z.x - zn.x);
       double pa = ar * ar + ai * ai, pb = br * br + bi * bi;
       if (p.power == 1) { pa = sqrt(pa); pb = sqrt(pb); }
+      if (p.spec_mult != 1.0) { pa *= p.spec_mult; pb *= p.spec_mult; }     // `normalized`
       P[k] = pa;
       P[NB + k] = pb;
     }

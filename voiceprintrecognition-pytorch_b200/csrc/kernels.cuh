@@ -9,6 +9,9 @@ struct FrontendParams {
   const float* window; const double2* twiddle;   // twiddle[k] = exp(-2 pi i k / N) in fp64
   const int* mel_start; const int* mel_count; const int* mel_off; const float* mel_w;
   int B, L, T, kind, N, WL, hop, F, remove_dc, power, use_log, fpb, nblk;
+  int frame;           // VP_FRAME_* of vp_frontend_options
+  int pad;             // kind 0 reflect: samples before x[0] (win/2 - hop/2, may be < 0); kind 1: torchaudio's zero pad
+  double spec_mult;    // multiplies |X|^power: spec_scale^power (1.0 = none)
   float preemph, log_floor, db_mult;
   float* cta_max;      // non-null: MFCC mel stage (per-CTA maxima instead of CMN partial sums)
   int n_pass, radix[12], G;   // FFT pass plan + threads per FFT group (frontend_plan)

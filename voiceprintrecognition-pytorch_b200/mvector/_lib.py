@@ -26,6 +26,14 @@ class FrontendDesc(C.Structure):
                 ('db_mult', C.c_float), ('top_db', C.c_float)]
 
 
+FRAME_DEFAULT, FRAME_KALDI_REFLECT, FRAME_STFT_CONSTANT, FRAME_STFT_REPLICATE, FRAME_STFT_CIRCULAR = 0, 1, 2, 3, 4
+FRAME_STFT_NOCENTER = 5
+
+
+class FrontendOptions(C.Structure):
+    _fields_ = [('frame_mode', C.c_int32), ('pad', C.c_int32), ('spec_scale', C.c_double)]
+
+
 class Op(C.Structure):
     _fields_ = ([('kind', C.c_int32), ('mode', C.c_int32), ('engine', C.c_int32), ('B', C.c_int32)]
                 + [(n, C.c_int64) for n in ('src', 'src2', 'dst', 'res', 'gate', 'ubias',
@@ -69,11 +77,13 @@ def lib():
         'vp_abi_version': (C.c_int, []),
         'vp_sizeof_op': (i32, []),
         'vp_sizeof_frontend_desc': (i32, []),
+        'vp_sizeof_frontend_options': (i32, []),
         'vp_create': (C.c_int, [C.c_int, pp]),
         'vp_destroy': (None, [vp]),
         'vp_last_error': (C.c_char_p, [vp]),
         'vp_frontend_set': (C.c_int, [vp, C.POINTER(FrontendDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, i32, C.c_void_p]),
+        'vp_frontend_set_options': (C.c_int, [vp, C.POINTER(FrontendOptions)]),
         'vp_feature_dim': (i32, [vp]),
         'vp_num_frames': (i32, [vp, i32]),
         'vp_frontend_scratch_floats': (sz, [vp, i32, i32]),
@@ -112,14 +122,16 @@ def lib():
         fn.argtypes = args
     if L.vp_abi_version() != 4:
         raise RuntimeError('libvpb200.so ABI version mismatch')
-    if L.vp_sizeof_op() != C.sizeof(Op) or L.vp_sizeof_frontend_desc() != C.sizeof(FrontendDesc):
-        raise RuntimeError('vp_op / vp_frontend_desc layout mismatch between the ctypes binding and libvpb200.so')
+    if L.vp_sizeof_op() != C.sizeof(Op) or L.vp_sizeof_frontend_desc() != C.sizeof(FrontendDesc) \
+            or L.vp_sizeof_frontend_options() != C.sizeof(FrontendOptions):
+        raise RuntimeError('vp_op / vp_frontend_desc / vp_frontend_options layout mismatch between the ctypes binding '
+                           'and libvpb200.so')
     _lib = L
     return L
 
 
 EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_create', 'vp_destroy', 'vp_last_error',
-           'vp_frontend_set', 'vp_num_frames', 'vp_frontend_scratch_floats', 'vp_fbank', 'vp_melspec', 'vp_mfcc',
+           'vp_frontend_set', 'vp_sizeof_frontend_options', 'vp_frontend_set_options', 'vp_num_frames', 'vp_frontend_scratch_floats', 'vp_fbank', 'vp_melspec', 'vp_mfcc',
            'vp_feature_dim',
            'vp_weights_load', 'vp_program_create', 'vp_program_destroy', 'vp_embed', 'vp_embed_wave',
            'vp_program_launches', 'vp_program_peek', 'vp_embed_profiled', 'vp_program_op_info', 'vp_host_gather_pad',

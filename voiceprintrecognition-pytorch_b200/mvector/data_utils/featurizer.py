@@ -40,15 +40,6 @@ def _fft_size_ok(n):
     return n == 1
 
 
-def _stft_window(n_fft, win_length):
-    """Periodic Hann of win_length taps, centred inside n_fft like torch.stft does for a short window."""
-    win = torch.hann_window(win_length)
-    if win_length < n_fft:
-        left = (n_fft - win_length) // 2
-        win = torch.nn.functional.pad(win, (left, n_fft - win_length - left))
-    return win.numpy().astype(np.float32)
-
-
 def _sparse_bank(dense):
     """dense [n_filters, n_bins] -> (start, count, offset, weights) over each filter's non-zero support."""
     start, count, off, w = [], [], [], []
@@ -64,9 +55,156 @@ def _sparse_bank(dense):
             np.asarray(w if w else [0.0], np.float32))
 
 
+def _unsupported(method, bad):
+    """Options outside the lowered front-end raise, each named with the reason: there is no CPU fallback."""
+    if bad:
+        raise NotImplementedError(f'{method} options not lowered to the sm_90a front-end: ' + '; '.join(bad))
+
+
+_FFT_SIZES = 'the FFT handles 2^a 3^b 5^c, a multiple of 4, in [64, 2048]'
+
+
+def _stft_window(n_fft, win_length, window_fn=torch.hann_window, wkwargs=None):
+    """window_fn(win_length, **wkwargs) (torchaudio's Spectrogram; periodic Hann by default), centred inside n_fft like
+    torch.stft does for a short window.  -> (the n_fft taps, the win_length taps before the padding)."""
+    taps = (window_fn(win_length) if wkwargs is None else window_fn(win_length, **wkwargs)).to(torch.float32)
+    win = taps
+    if win_length < n_fft:
+        left = (n_fft - win_length) // 2
+        win = torch.nn.functional.pad(win, (left, n_fft - win_length - left))
+    return win.numpy().astype(np.float32), taps
+
+
+_PAD_MODES = {'reflect': L.FRAME_DEFAULT, 'constant': L.FRAME_STFT_CONSTANT, 'replicate': L.FRAME_STFT_REPLICATE,
+              'circular': L.FRAME_STFT_CIRCULAR}
+
+
+def _stft_options(a, n_fft, taps):
+    """Framing and scale of torchaudio's spectrogram (functional.py:52-144): zeros `pad` (> 0 only) at both ends, then
+    torch.stft centring by n_fft/2 in `pad_mode` (none when center=False), and |X| scaled by 1/sqrt(sum(window^2))
+    (normalized True / 'window') or by 1/sqrt(n_fft) (normalized 'frame_length', torch.stft's own normalisation)."""
+    normalized = a['normalized']
+    if isinstance(normalized, str):
+        if normalized not in ('frame_length', 'window'):
+            raise ValueError('Invalid normalized parameter: {}'.format(normalized))
+    elif not isinstance(normalized, bool):
+        raise TypeError('Input type not supported')
+    if normalized == 'frame_length':
+        scale = 1.0 / math.sqrt(n_fft)
+    elif normalized is True or normalized == 'window':
+        scale = 1.0 / float(taps.pow(2.0).sum().sqrt())      # the fp32 norm the reference divides by
+    else:
+        scale = 1.0
+    if not a['center']:
+        mode = L.FRAME_STFT_NOCENTER
+    elif a['pad_mode'] in _PAD_MODES:
+        mode = _PAD_MODES[a['pad_mode']]
+    else:
+        raise NotImplementedError('Unrecognised padding mode ' + str(a['pad_mode']))
+    return L.FrontendOptions(frame_mode=mode, pad=max(int(a['pad']), 0), spec_scale=scale)
+
+
+def _hz_to_mel(f, mel_scale):
+    """functional._hz_to_mel (functional.py:425-456), python floats."""
+    if mel_scale == 'htk':
+        return 2595.0 * math.log10(1.0 + (f / 700.0))
+    mels = f / (200.0 / 3)
+    if f >= 1000.0:
+        mels = 1000.0 / (200.0 / 3) + math.log(f / 1000.0) / (math.log(6.4) / 27.0)
+    return mels
+
+
+def _mel_to_hz(mels, mel_scale):
+    """functional._mel_to_hz (functional.py:459-489), fp32 tensor."""
+    if mel_scale == 'htk':
+        return 700.0 * (10.0 ** (mels / 2595.0) - 1.0)
+    min_log_mel, logstep = 1000.0 / (200.0 / 3), math.log(6.4) / 27.0
+    freqs = 0.0 + (200.0 / 3) * mels
+    log_t = mels >= min_log_mel
+    freqs[log_t] = 1000.0 * torch.exp(logstep * (mels[log_t] - min_log_mel))
+    return freqs
+
+
+def melscale_fbanks(n_freqs, f_min, f_max, n_mels, sample_rate, norm=None, mel_scale='htk'):
+    """functional.melscale_fbanks (functional.py:518-587): HTK or Slaney mel scale, optional Slaney area normalisation.
+    Returns [n_freqs, n_mels] float32."""
+    if norm is not None and norm != 'slaney':
+        raise ValueError('norm must be one of None or "slaney"')
+    if mel_scale not in ('htk', 'slaney'):
+        raise ValueError('mel_scale should be one of "htk" or "slaney".')
+    all_freqs = torch.linspace(0, sample_rate // 2, n_freqs)
+    f_pts = _mel_to_hz(torch.linspace(_hz_to_mel(f_min, mel_scale), _hz_to_mel(f_max, mel_scale), n_mels + 2),
+                       mel_scale)
+    f_diff = f_pts[1:] - f_pts[:-1]
+    slopes = f_pts.unsqueeze(0) - all_freqs.unsqueeze(1)
+    fb = torch.max(torch.zeros(1), torch.min((-1.0 * slopes[:, :-2]) / f_diff[:-1], slopes[:, 2:] / f_diff[1:]))
+    if norm == 'slaney':
+        fb *= (2.0 / (f_pts[2:n_mels + 2] - f_pts[:n_mels])).unsqueeze(0)
+    return fb
+
+
+def _kaldi_mel(f):
+    return 1127.0 * (1.0 + f / 700.0).log()
+
+
+def _vtln_warp_freq(vtln_low, vtln_high, low_freq, high_freq, warp, freq):
+    """kaldi.vtln_warp_freq (kaldi.py:334-406): identity outside [low_freq, high_freq], freq / warp between the
+    inflection points l = vtln_low * max(1, warp) and h = vtln_high * min(1, warp), linear in between."""
+    assert vtln_low > low_freq, 'be sure to set the vtln_low option higher than low_freq'
+    assert vtln_high < high_freq, 'be sure to set the vtln_high option lower than high_freq [or negative]'
+    lo, hi = vtln_low * max(1.0, warp), vtln_high * min(1.0, warp)
+    scale = 1.0 / warp
+    assert lo > low_freq and hi < high_freq
+    scale_left = (scale * lo - low_freq) / (lo - low_freq)
+    scale_right = (high_freq - scale * hi) / (high_freq - hi)
+    res = torch.empty_like(freq)
+    outside = torch.lt(freq, low_freq) | torch.gt(freq, high_freq)
+    before_l, before_h, after_h = torch.lt(freq, lo), torch.lt(freq, hi), torch.ge(freq, hi)
+    res[after_h] = high_freq + scale_right * (freq[after_h] - high_freq)       # later masks overwrite earlier ones
+    res[before_h] = scale * freq[before_h]
+    res[before_l] = low_freq + scale_left * (freq[before_l] - low_freq)
+    res[outside] = freq[outside]
+    return res
+
+
+def kaldi_mel_banks(n_mels, n_fft, sf, low_freq, high_freq, vtln_low=100.0, vtln_high=-500.0, vtln_warp=1.0):
+    """kaldi.get_mel_banks (kaldi.py:436-511), VTLN-warped when vtln_warp != 1.  Returns [n_mels, n_fft // 2] float32."""
+    nyq = 0.5 * sf
+    if high_freq <= 0.0:
+        high_freq += nyq
+    assert 0.0 <= low_freq < nyq and 0.0 < high_freq <= nyq and low_freq < high_freq, \
+        'Bad values in options: low-freq / high-freq'
+    bw = sf / n_fft
+    mlo, mhi = 1127.0 * math.log(1.0 + low_freq / 700.0), 1127.0 * math.log(1.0 + high_freq / 700.0)
+    delta = (mhi - mlo) / (n_mels + 1)
+    if vtln_high < 0.0:
+        vtln_high += nyq
+    assert vtln_warp == 1.0 or (low_freq < vtln_low < high_freq and 0.0 < vtln_high < high_freq
+                                and vtln_low < vtln_high), 'Bad values in options: vtln-low / vtln-high'
+    b = torch.arange(n_mels).unsqueeze(1)
+    left, center, right = mlo + b * delta, mlo + (b + 1.0) * delta, mlo + (b + 2.0) * delta
+    if vtln_warp != 1.0:
+        left, center, right = (_kaldi_mel(_vtln_warp_freq(vtln_low, vtln_high, low_freq, high_freq, vtln_warp,
+                                                          700.0 * ((x / 1127.0).exp() - 1.0)))
+                               for x in (left, center, right))
+    mel = _kaldi_mel(bw * torch.arange(n_fft / 2)).unsqueeze(0)
+    up, down = (mel - left) / (center - left), (right - mel) / (right - center)
+    if vtln_warp == 1.0:
+        return torch.max(torch.zeros(1), torch.min(up, down))
+    banks = torch.zeros_like(up)                          # warping can reorder left / center / right
+    up_idx = torch.gt(mel, left) & torch.le(mel, center)
+    down_idx = torch.gt(mel, center) & torch.lt(mel, right)
+    banks[up_idx] = up[up_idx]
+    banks[down_idx] = down[down_idx]
+    return banks
+
+
 class KaldiFbank:
     """kwargs of torchaudio.compliance.kaldi.fbank (featurizer.py:114-117); constants follow kaldi.py:86-113
-    (window) and kaldi.py:436-511 (mel banks), evaluated once in fp32 with the same torch ops."""
+    (window) and kaldi.py:436-511 (mel banks, VTLN-warped or not), evaluated once in fp32 with the same torch ops.
+    snip_edges=False frames the half-sample-reflected signal (kaldi.py:44-83); round_to_power_of_two=False runs an FFT of
+    the window's own length; subtract_mean needs nothing: AudioFeaturizer.forward subtracts the column mean again right
+    after it, so the reference's result differs from plain CMN by rounding only."""
 
     def __init__(self, **kwargs):
         for k in kwargs:
@@ -75,18 +213,27 @@ class KaldiFbank:
         a = dict(_FBANK_DEFAULTS)
         a.update(kwargs)
         self.kwargs = kwargs
-        unsupported = [k for k, bad in (('dither', a['dither'] != 0.0), ('vtln_warp', a['vtln_warp'] != 1.0),
-                                        ('snip_edges', not a['snip_edges']), ('use_energy', a['use_energy']),
-                                        ('subtract_mean', a['subtract_mean']),
-                                        ('min_duration', a['min_duration'] != 0.0),
-                                        ('round_to_power_of_two', not a['round_to_power_of_two']),
-                                        ('channel', a['channel'] not in (-1, 0))) if bad]
-        if unsupported:
-            raise NotImplementedError('Fbank options not lowered to the sm_90a front-end: ' + ', '.join(unsupported))
         sf = a['sample_frequency']
         self.hop = int(sf * a['frame_shift'] * 0.001)
         self.win_length = int(sf * a['frame_length'] * 0.001)
-        self.n_fft = 1 if self.win_length == 0 else 2 ** (self.win_length - 1).bit_length()
+        if a['round_to_power_of_two']:
+            self.n_fft = 1 if self.win_length == 0 else 2 ** (self.win_length - 1).bit_length()
+        else:
+            self.n_fft = self.win_length
+        bad = []
+        if a['dither'] != 0.0:
+            bad.append(f"dither={a['dither']} (the reference draws fresh random noise on every call)")
+        if a['min_duration'] != 0.0:
+            bad.append(f"min_duration={a['min_duration']} (the reference returns an empty tensor for a shorter "
+                       "utterance, which its torch.stack of the batch cannot take)")
+        if a['channel'] not in (-1, 0):
+            bad.append(f"channel={a['channel']} (the reference passes one mono row per utterance)")
+        if a['use_energy']:
+            bad.append('use_energy=True (the energy column is not counted by feature_dim, so no model consumes it; '
+                       'raw_energy, energy_floor and htk_compat act only with it)')
+        if not a['round_to_power_of_two'] and not _fft_size_ok(self.n_fft):
+            bad.append(f'round_to_power_of_two=False with a {self.win_length}-sample window ({_FFT_SIZES})')
+        _unsupported('Fbank', bad)
         self.n_mels = a['num_mel_bins']
         assert self.n_mels > 3, 'Must have at least 3 mel bins'
         wt = a['window_type']
@@ -106,61 +253,55 @@ class KaldiFbank:
         else:
             raise Exception('Invalid window type ' + wt)
         self.window = win.numpy().astype(np.float32)
-        # mel banks
-        nyq = 0.5 * sf
-        lo, hi = a['low_freq'], a['high_freq']
-        if hi <= 0.0:
-            hi += nyq
-        assert 0.0 <= lo < nyq and 0.0 < hi <= nyq and lo < hi, 'Bad values in options: low-freq / high-freq'
-        bw = sf / self.n_fft
-        mlo, mhi = 1127.0 * math.log(1.0 + lo / 700.0), 1127.0 * math.log(1.0 + hi / 700.0)
-        delta = (mhi - mlo) / (self.n_mels + 1)
-        b = torch.arange(self.n_mels).unsqueeze(1)
-        left, center, right = mlo + b * delta, mlo + (b + 1.0) * delta, mlo + (b + 2.0) * delta
-        mel = (1127.0 * (1.0 + (bw * torch.arange(self.n_fft / 2)) / 700.0).log()).unsqueeze(0)
-        banks = torch.max(torch.zeros(1), torch.min((mel - left) / (center - left), (right - mel) / (right - center)))
+        banks = kaldi_mel_banks(self.n_mels, self.n_fft, sf, a['low_freq'], a['high_freq'], a['vtln_low'],
+                                a['vtln_high'], a['vtln_warp'])
         self.bank = _sparse_bank(banks.to(torch.float32).numpy())   # bin n_fft/2 has weight 0 (kaldi.py:627)
         self.desc = L.FrontendDesc(kind=0, n_fft=self.n_fft, win_length=self.win_length, hop=self.hop,
                                    n_mels=self.n_mels, remove_dc=1 if a['remove_dc_offset'] else 0,
                                    preemph=float(a['preemphasis_coefficient']), power=2 if a['use_power'] else 1,
                                    use_log=1 if a['use_log_fbank'] else 0, log_floor=float(np.finfo(np.float32).eps))
+        self.opts = L.FrontendOptions(frame_mode=L.FRAME_DEFAULT if a['snip_edges'] else L.FRAME_KALDI_REFLECT, pad=0,
+                                      spec_scale=1.0)
+
+
+def _stft_args(defaults, name, kwargs):
+    for k in kwargs:
+        if k not in defaults and k not in ('window_fn', 'wkwargs'):
+            raise TypeError(f"{name}.__init__() got an unexpected keyword argument '{k}'")
+    a = dict(defaults)
+    a.update(kwargs)
+    n_fft = a['n_fft']
+    win_length = a['win_length'] if a['win_length'] is not None else n_fft
+    hop = a['hop_length'] if a['hop_length'] is not None else win_length // 2
+    bad = []
+    if a['power'] not in (1.0, 2.0, 1, 2):
+        bad.append(f"power={a['power']} (|X| and |X|^2 are lowered)")
+    if not _fft_size_ok(n_fft):
+        bad.append(f'n_fft={n_fft} ({_FFT_SIZES})')
+    if win_length > n_fft:
+        bad.append(f'win_length={win_length} (longer than n_fft)')
+    return a, n_fft, win_length, hop, bad
 
 
 class MelSpectrogram:
-    """kwargs of torchaudio.transforms.MelSpectrogram (featurizer.py:41-42): periodic Hann, centred reflect-padded
-    STFT (functional.py:123-135), |X|^power, HTK triangular bank (functional.py:518-587).  No log (featurizer.py:76)."""
+    """kwargs of torchaudio.transforms.MelSpectrogram (featurizer.py:41-42): window_fn (periodic Hann by default), STFT
+    framing of _stft_options, |X|^power, HTK or Slaney triangular bank (functional.py:518-587).  No log
+    (featurizer.py:76)."""
 
     def __init__(self, **kwargs):
-        for k in kwargs:
-            if k not in _MELSPEC_DEFAULTS and k not in ('window_fn', 'wkwargs'):
-                raise TypeError(f"MelSpectrogram.__init__() got an unexpected keyword argument '{k}'")
-        a = dict(_MELSPEC_DEFAULTS)
-        a.update(kwargs)
+        a, n_fft, win_length, hop, bad = _stft_args(_MELSPEC_DEFAULTS, 'MelSpectrogram', kwargs)
         self.kwargs = kwargs
-        n_fft = a['n_fft']
-        win_length = a['win_length'] if a['win_length'] is not None else n_fft
-        hop = a['hop_length'] if a['hop_length'] is not None else win_length // 2
         f_max = a['f_max'] if a['f_max'] is not None else float(a['sample_rate'] // 2)
-        bad = [k for k, b in (('window_fn', 'window_fn' in kwargs or 'wkwargs' in kwargs), ('pad', a['pad'] != 0),
-                              ('normalized', bool(a['normalized'])), ('center', not a['center']),
-                              ('pad_mode', a['pad_mode'] != 'reflect'), ('norm', a['norm'] is not None),
-                              ('mel_scale', a['mel_scale'] != 'htk'), ('power', a['power'] not in (1.0, 2.0, 1, 2)),
-                              ('n_fft (2^a 3^b 5^c, multiple of 4, in [64, 2048])', not _fft_size_ok(n_fft)),
-                              ('n_mels (<= 128)', a['n_mels'] > 128),
-                              ('win_length', win_length > n_fft)) if b]
-        if bad:
-            raise NotImplementedError('MelSpectrogram options not lowered to the sm_90a front-end: ' + ', '.join(bad))
+        if a['n_mels'] > n_fft // 2 + 1:
+            bad.append(f"n_mels={a['n_mels']} (at most n_fft/2 + 1 = {n_fft // 2 + 1} filters)")
+        _unsupported('MelSpectrogram', bad)
         self.n_fft, self.hop, self.n_mels = n_fft, hop, a['n_mels']
-        self.window = _stft_window(n_fft, win_length)
+        self.window, taps = _stft_window(n_fft, win_length, kwargs.get('window_fn', torch.hann_window),
+                                         kwargs.get('wkwargs'))
+        self.opts = _stft_options(a, n_fft, taps)
         self.win_length = n_fft
-        n_freqs = n_fft // 2 + 1
-        all_freqs = torch.linspace(0, a['sample_rate'] // 2, n_freqs)
-        m_min = 2595.0 * math.log10(1.0 + (a['f_min'] / 700.0))
-        m_max = 2595.0 * math.log10(1.0 + (f_max / 700.0))
-        f_pts = 700.0 * (10.0 ** (torch.linspace(m_min, m_max, self.n_mels + 2) / 2595.0) - 1.0)
-        f_diff = f_pts[1:] - f_pts[:-1]
-        slopes = f_pts.unsqueeze(0) - all_freqs.unsqueeze(1)
-        fb = torch.max(torch.zeros(1), torch.min((-1.0 * slopes[:, :-2]) / f_diff[:-1], slopes[:, 2:] / f_diff[1:]))
+        fb = melscale_fbanks(n_fft // 2 + 1, a['f_min'], f_max, self.n_mels, a['sample_rate'], a['norm'],
+                             a['mel_scale'])
         self.bank = _sparse_bank(fb.T.contiguous().numpy())
         self.desc = L.FrontendDesc(kind=1, n_fft=n_fft, win_length=n_fft, hop=hop, n_mels=self.n_mels, remove_dc=0,
                                    preemph=0.0, power=int(a['power']), use_log=0, log_floor=0.0)
@@ -173,26 +314,17 @@ class Spectrogram:
     projection -- the "bank" is the identity over the n_fft/2+1 bins, so the same kernel emits |X|^power directly."""
 
     def __init__(self, **kwargs):
-        for k in kwargs:
-            if k not in _SPEC_DEFAULTS and k not in ('window_fn', 'wkwargs'):
-                raise TypeError(f"Spectrogram.__init__() got an unexpected keyword argument '{k}'")
-        a = dict(_SPEC_DEFAULTS)
-        a.update(kwargs)
+        a, n_fft, win_length, hop, bad = _stft_args(_SPEC_DEFAULTS, 'Spectrogram', kwargs)
         self.kwargs = kwargs
-        n_fft = a['n_fft']
-        win_length = a['win_length'] if a['win_length'] is not None else n_fft
-        hop = a['hop_length'] if a['hop_length'] is not None else win_length // 2
-        bad = [k for k, b in (('window_fn', 'window_fn' in kwargs or 'wkwargs' in kwargs), ('pad', a['pad'] != 0),
-                              ('normalized', bool(a['normalized'])), ('center', not a['center']),
-                              ('pad_mode', a['pad_mode'] != 'reflect'), ('onesided', not a['onesided']),
-                              ('power', a['power'] not in (1.0, 2.0, 1, 2)),
-                              ('n_fft (2^a 3^b 5^c, multiple of 4, in [64, 2048])', not _fft_size_ok(n_fft)),
-                              ('win_length', win_length > n_fft)) if b]
-        if bad:
-            raise NotImplementedError('Spectrogram options not lowered to the sm_90a front-end: ' + ', '.join(bad))
+        if not a['onesided']:
+            bad.append('onesided=False (feature_dim counts n_fft/2 + 1 bins, so no model consumes the two-sided '
+                       'spectrum)')
+        _unsupported('Spectrogram', bad)
         nb = n_fft // 2 + 1
         self.n_fft, self.hop, self.n_mels = n_fft, hop, nb
-        self.window = _stft_window(n_fft, win_length)
+        self.window, taps = _stft_window(n_fft, win_length, kwargs.get('window_fn', torch.hann_window),
+                                         kwargs.get('wkwargs'))
+        self.opts = _stft_options(a, n_fft, taps)
         self.win_length = n_fft
         idx = np.arange(nb, dtype=np.int32)
         self.bank = (idx, np.ones(nb, np.int32), idx.copy(), np.ones(nb, np.float32))
@@ -219,8 +351,10 @@ class MFCC:
         n_mfcc, n_mels = a['n_mfcc'], mel.n_mels
         if n_mfcc > n_mels:
             raise ValueError('Cannot select more MFCC coefficients than # mel bins')
+        _unsupported('MFCC', [f'n_mels={n_mels} (the DCT stage keeps its matrix in shared memory: at most 128 mel '
+                              'bins)'] if n_mels > 128 else [])
         self.n_fft, self.hop, self.n_mels, self.win_length = mel.n_fft, mel.hop, n_mels, mel.win_length
-        self.window, self.bank = mel.window, mel.bank
+        self.window, self.bank, self.opts = mel.window, mel.bank, mel.opts
         n = torch.arange(float(n_mels))
         k = torch.arange(float(n_mfcc)).unsqueeze(1)
         dct = torch.cos(math.pi / float(n_mels) * (n + 0.5) * k)
@@ -283,6 +417,7 @@ class AudioFeaturizer:
             self._engine.handle, C.byref(f.desc), win.ctypes.data_as(C.c_void_p), start.ctypes.data_as(C.c_void_p),
             count.ctypes.data_as(C.c_void_p), off.ctypes.data_as(C.c_void_p), w.ctypes.data_as(C.c_void_p), int(w.size),
             dct.ctypes.data_as(C.c_void_p) if dct is not None else C.c_void_p()))
+        _check(self._engine.handle, L.lib().vp_frontend_set_options(self._engine.handle, C.byref(f.opts)))
         self._configured = True
 
     @property
@@ -291,10 +426,18 @@ class AudioFeaturizer:
         return self._engine
 
     def num_frames(self, n_samples):
+        """Frames T for a waveform of n_samples (vp_num_frames): kaldi._get_strided, or torch.stft of the `pad`-extended
+        signal, centred or not."""
         f = self.feat_fun
+        mode = f.opts.frame_mode
         if f.desc.kind == 0:
+            if mode == L.FRAME_KALDI_REFLECT:
+                return (n_samples + f.hop // 2) // f.hop
             return 0 if n_samples < f.win_length else 1 + (n_samples - f.win_length) // f.hop
-        return 1 + n_samples // f.hop
+        n = n_samples + 2 * f.opts.pad
+        if mode == L.FRAME_STFT_NOCENTER:
+            return 0 if n < f.n_fft else 1 + (n - f.n_fft) // f.hop
+        return 1 + n // f.hop
 
     @staticmethod
     def keep_frames(input_lens_ratio, T):
