@@ -322,6 +322,36 @@ int vp_verify_metrics(vp_handle* h, const float* scores, int64_t n, const int32_
                       double c_fa, void* scratch, float* sorted_scores, uint8_t* sorted_labels, vp_verify_result* result,
                       void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Input conditioning of _load_audio (predict.py:185-212) on the device: resample to the model's rate, then dB-normalise.
+ * ---------------------------------------------------------------------------------------------------------- */
+/* Polyphase resampler: row b of out [B, out_ld] <- scipy.signal.resample_poly(in[b, :n_in[b]].astype(float64),
+ * up[b], down[b]) (window ('kaiser', 5.0), padtype 'constant') rounded to float32; columns >= n_out[b] are written as 0.
+ * n_out[b] must be ceil(n_in[b] * up[b] / down[b]) (in int64) and <= out_ld; up[b] == down[b] copies the row.
+ * With max_rate = max(up, down), half_len = 10 max_rate, h = firwin(2 half_len + 1, 1 / max_rate, ('kaiser', 5.0)) * up,
+ * n_pre_pad = down - half_len % down, hpad = (n_pre_pad zeros, h), Lh = len(hpad), nt = ceil(Lh / up) and
+ * n_pre_remove = (half_len + n_pre_pad) / down, taps[tap_off[b] + p * nt + m] = hpad[p + m * up] (0 past Lh) for every
+ * phase 0 <= p < up (float64, device; the host designs it once per (up, down)).  Output j is upfirdn output
+ * i = j + n_pre_remove: acc = 0.0, then for k = max(0, ceil((i down - (Lh - 1)) / up)) .. min(n_in - 1, floor(i down / up))
+ * in increasing order acc = __dadd_rn(acc, __dmul_rn((double)in[k], hpad[i down - k up])), one rounding to float32 at the
+ * end: scipy's operation order, so the result is bit-identical.  n_in, n_out, tap_off int64 [B], up, down int32 [B],
+ * all device.  in and out must not overlap.  Asynchronous on stream. */
+int vp_resample(vp_handle* h, const float* in, int64_t in_ld, float* out, int64_t out_ld, int32_t B, const int64_t* n_in,
+                const int64_t* n_out, const int32_t* up, const int32_t* down, const int64_t* tap_off, const double* taps,
+                void* stream);
+/* device scratch bytes vp_gain_normalize needs for B rows of leading dimension ld */
+size_t vp_gain_scratch_bytes(const vp_handle* h, int32_t B, int64_t ld);
+/* In place on wave [B, ld] (device float32), the twin of AudioSegment.normalize(target_db, max_gain_db) on
+ * wave[b, :lens[b]] (lens int64 [B], device): mean = sum x^2 / n in float64 (per-tile sums of the exact squares combined
+ * in tile order), gain = target_db - 10 log10(mean), factor = 10^(gain / 20) in float64 and x <- (float)(x * factor),
+ * the float64 product numpy forms for a float32 array times a float64 scalar.  log10 / pow are CUDA's (<= 2 ulp from
+ * glibc's), so a factor may differ from the host's in the last float64 bits; an output sample then differs by at most
+ * one float32 ulp, and only when x * factor lies next to a float32 rounding boundary.  flags[b] (int32, device) <- 1
+ * when gain > max_gain_db (a silent row: gain +inf), the row then left unscaled; else 0.  NaN samples give a NaN row,
+ * as on the host.  Columns >= lens[b] are not touched.  Asynchronous on stream; no atomics. */
+int vp_gain_normalize(vp_handle* h, float* wave, int64_t ld, int32_t B, const int64_t* lens, double target_db,
+                      double max_gain_db, int32_t* flags, void* scratch, void* stream);
+
 /* Staging half of predict_batch (predict.py:244-255) as ONE native call: worker threads gather slices of slice_rows
  * utterances into the zero-padded PINNED matrix staging[n, lmax]; the calling thread -- one of the n_threads gatherers --
  * issues cudaMemcpyAsync(staging slice -> device_dst slice) on copy_stream, in slice order, as soon as a slice is

@@ -862,6 +862,35 @@ int vp_verify_metrics(vp_handle* h, const float* scores, int64_t n, const int32_
   return VP_OK;
 }
 
+int vp_resample(vp_handle* h, const float* in, int64_t in_ld, float* out, int64_t out_ld, int32_t B, const int64_t* n_in,
+                const int64_t* n_out, const int32_t* up, const int32_t* down, const int64_t* tap_off, const double* taps,
+                void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (B < 0 || B > 65535) return fail(h, VP_ERR_UNSUPPORTED, "B = %d outside [0, 65535]", B);
+  if (B == 0 || out_ld == 0) return VP_OK;
+  if (!in || !out || !n_in || !n_out || !up || !down || !tap_off || !taps || in_ld < 0 || out_ld < 0)
+    return fail(h, VP_ERR_INVALID, "null argument or negative leading dimension");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_resample(in, in_ld, out, out_ld, B, n_in, n_out, up, down, tap_off, taps, (cudaStream_t)stream));
+  return VP_OK;
+}
+
+size_t vp_gain_scratch_bytes(const vp_handle* h, int32_t B, int64_t ld) {
+  (void)h;
+  return B < 1 || ld < 0 ? 0 : gain_scratch_bytes(B, ld);
+}
+
+int vp_gain_normalize(vp_handle* h, float* wave, int64_t ld, int32_t B, const int64_t* lens, double target_db,
+                      double max_gain_db, int32_t* flags, void* scratch, void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (B < 0 || B > 65535) return fail(h, VP_ERR_UNSUPPORTED, "B = %d outside [0, 65535]", B);
+  if (B == 0) return VP_OK;
+  if (!wave || !lens || !flags || !scratch || ld < 1) return fail(h, VP_ERR_INVALID, "null/empty argument");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_gain(wave, ld, B, lens, target_db, max_gain_db, flags, scratch, (cudaStream_t)stream));
+  return VP_OK;
+}
+
 int vp_program_peek(vp_program* p, int64_t off, size_t nbytes, void* dst, void* stream) {
   if (!p || !dst) return VP_ERR_INVALID;
   if (off < 0 || (size_t)off + nbytes > p->ws_bytes) return fail(p->h, VP_ERR_INVALID, "peek out of range");

@@ -70,6 +70,14 @@ cudaError_t launch_verify_sort(const float* scores, const int32_t* labels, const
 cudaError_t launch_verify_curve(int64_t n, double p_target, double c_miss, double c_fa, void* scratch, float* sorted_scores,
                                 uint8_t* sorted_labels, vp_verify_result* result, cudaStream_t stream);
 
+// input conditioning: polyphase resampler and dB gain (condition.cu)
+cudaError_t launch_resample(const float* x, int64_t in_ld, float* y, int64_t out_ld, int B, const int64_t* n_in,
+                            const int64_t* n_out, const int32_t* up, const int32_t* down, const int64_t* tap_off,
+                            const double* taps, cudaStream_t stream);
+size_t gain_scratch_bytes(int B, int64_t ld);
+cudaError_t launch_gain(float* w, int64_t ld, int B, const int64_t* lens, double target_db, double max_gain_db,
+                        int32_t* flags, void* scratch, cudaStream_t stream);
+
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);

@@ -115,6 +115,11 @@ def lib():
         'vp_verify_scratch_bytes': (sz, [vp, C.c_int64]),
         'vp_verify_metrics': (C.c_int, [vp, f32p, C.c_int64, i32p, i32p, C.c_int64, i32p, C.c_int64, C.c_double,
                                         C.c_double, C.c_double, C.c_void_p, f32p, C.c_void_p, C.c_void_p, vp]),
+        'vp_resample': (C.c_int, [vp, f32p, C.c_int64, f32p, C.c_int64, i32, C.c_void_p, C.c_void_p, C.c_void_p,
+                                  C.c_void_p, C.c_void_p, C.c_void_p, vp]),
+        'vp_gain_scratch_bytes': (sz, [vp, i32, C.c_int64]),
+        'vp_gain_normalize': (C.c_int, [vp, f32p, C.c_int64, i32, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
+                                        C.c_void_p, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = header/library mismatch
@@ -137,4 +142,5 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_program_launches', 'vp_program_peek', 'vp_embed_profiled', 'vp_program_op_info', 'vp_host_gather_pad',
            'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_cosine_scores', 'vp_device_zero',
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
-           'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics']
+           'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics',
+           'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize']

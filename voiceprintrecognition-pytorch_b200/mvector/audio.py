@@ -5,8 +5,40 @@ from this image; decoding/resampling sit OUTSIDE the parity boundary (SURVEY.md 
 waveforms).  Decoding covers PCM WAV via the standard library only."""
 import io
 import wave
+from math import gcd
 
 import numpy as np
+
+
+def resample_ratio(sample_rate, target_rate):
+    """(up, down) of ``AudioSegment.resample`` from ``sample_rate`` to ``target_rate``: the rates divided by their gcd."""
+    g = gcd(int(target_rate), int(sample_rate))
+    return int(target_rate) // g, int(sample_rate) // g
+
+
+def resampled_length(n, up, down):
+    """Samples resample_poly returns for n input samples: ceil(n * up / down), in int64 (ten minutes at 44.1 kHz times
+    up = 160 does not fit in int32).  Works elementwise on arrays."""
+    return -(-np.asarray(n, dtype=np.int64) * np.asarray(up, dtype=np.int64) // np.asarray(down, dtype=np.int64))
+
+
+def polyphase_taps(up, down):
+    """resample_poly's anti-aliasing filter for (up, down), laid out per phase for the device resampler
+    (include/vpb200.h, vp_resample) -> (table float64 [up * nt], nt, n_pre_remove).
+
+    scipy's recipe: max_rate = max(up, down), half_len = 10 max_rate, h = firwin(2 half_len + 1, 1 / max_rate,
+    window=('kaiser', 5.0)) * up, n_pre_pad = down - half_len % down, n_pre_remove = (half_len + n_pre_pad) // down.
+    hpad = (n_pre_pad zeros, h); table[p * nt + m] = hpad[p + m * up], zero past the end of hpad."""
+    from scipy.signal import firwin
+    max_rate = max(up, down)
+    half_len = 10 * max_rate
+    h = firwin(2 * half_len + 1, 1.0 / max_rate, window=('kaiser', 5.0)) * up
+    n_pre_pad = down - half_len % down
+    hpad = np.concatenate([np.zeros(n_pre_pad), h])
+    nt = -(-len(hpad) // up)
+    flat = np.zeros(up * nt)
+    flat[:len(hpad)] = hpad
+    return np.ascontiguousarray(flat.reshape(nt, up).T).reshape(-1), nt, (half_len + n_pre_pad) // down
 
 
 class AudioSegment:
@@ -56,7 +88,6 @@ class AudioSegment:
     def resample(self, target_sample_rate):
         if target_sample_rate == self.sample_rate:
             return
-        from math import gcd
         from scipy.signal import resample_poly
         g = gcd(int(target_sample_rate), self.sample_rate)
         self.samples = resample_poly(self.samples.astype(np.float64), int(target_sample_rate) // g,

@@ -169,47 +169,58 @@ def predict_batch_sharded(predictor, audios_data, sample_rate=16000, group=None,
     """``MVectorPredictor.predict_batch`` (predict.py:231-265) over all ranks of ``group``: every rank passes the same
     list, loads / stages / embeds only its contiguous shard -- padded to the longest item of the WHOLE list, with the
     whole list's mask ratios -- and one all-gather returns ``[B, embd_dim]`` (order preserved) on every rank.  The result
-    is bit-identical to the single-process ``predict_batch`` of the same list."""
+    is bit-identical to the single-process ``predict_batch`` of the same list.
+
+    Lmax and the ratios need only the other ranks' lengths after resampling, which follow from their native lengths and
+    rates (``resampled_length``): a rank decodes its own shard and conditions it (resample, dB normalisation) on its
+    device, and never materialises another rank's waveforms."""
+    from .audio import resample_ratio, resampled_length
     rank, world = _world(group)
     n = len(audios_data)
     target_sr = predictor.configs.dataset_conf.dataset.sample_rate
     lo, hi = shard_range(n, rank, world)
     ds = predictor.configs.dataset_conf.dataset
-    raw = sample_rate == target_sr and not ds.get('use_dB_normalization', False)
     mine = {}
-    if n > 0 and sample_rate == target_sr and set(map(type, audios_data)) == {np.ndarray}:
-        # Raw arrays at the model's rate: Lmax needs only the lengths of the other ranks' items -- one C-level pass
+    rates = np.full(n, int(sample_rate), dtype=np.int64)
+    if n > 0 and set(map(type, audios_data)) == {np.ndarray}:
+        # Raw arrays at the caller's rate: Lmax needs only the lengths of the other ranks' items -- one C-level pass
         # (a Python loop over the WHOLE list costs ~2 us per item: 4 ms per call for 2048 utterances on 8 ranks, which was
         # the whole end-to-end scaling loss of the 8-GPU runs) -- and this rank's own items are used in place when
-        # _load_audio would hand them back unchanged (predict.py:196-211), else decoded like any other input
+        # _load_audio would hand them back unchanged (predict.py:196-204), else decoded like any other input
         lens = np.fromiter(map(len, audios_data), dtype=np.int64, count=n)
         short = int(lens.min())
         assert short / float(sample_rate) >= ds.min_duration, f'音频太短，最小应该为{ds.min_duration}s，当前音频为{short / float(sample_rate)}s'
         for i in range(lo, hi):
             a = audios_data[i]
-            if raw and a.dtype == np.float32 and a.ndim == 1 and a.flags.c_contiguous:
+            if a.dtype == np.float32 and a.ndim == 1 and a.flags.c_contiguous:
                 mine[i] = a
             else:
                 seg = predictor._load_audio(audio_data=a, sample_rate=sample_rate)
                 mine[i] = np.ascontiguousarray(seg.samples, dtype=np.float32)
                 lens[i] = mine[i].shape[0]
-        lens = lens.tolist()
     else:
-        lens = []
+        lens = np.empty(n, dtype=np.int64)
         for i, a in enumerate(audios_data):
-            if type(a) is np.ndarray and a.ndim == 1 and sample_rate == target_sr and not (lo <= i < hi):
+            if type(a) is np.ndarray and a.ndim == 1 and not (lo <= i < hi):
                 assert a.shape[0] / float(sample_rate) >= ds.min_duration, \
                     f'音频太短，最小应该为{ds.min_duration}s，当前音频为{a.shape[0] / float(sample_rate)}s'
-                lens.append(a.shape[0])             # another rank's raw array: only its length matters here
+                lens[i] = a.shape[0]                # another rank's raw array: only its length matters here
                 continue
             seg = predictor._load_audio(audio_data=a, sample_rate=sample_rate)
-            lens.append(seg.samples.shape[0])
+            lens[i] = seg.samples.shape[0]
+            if not isinstance(a, np.ndarray):
+                rates[i] = seg.sample_rate         # files, bytes and AudioSegments carry their own rate
             if lo <= i < hi:
                 mine[i] = np.ascontiguousarray(seg.samples, dtype=np.float32)
-    lmax = max(lens)
+    ratio = {r: resample_ratio(r, target_sr) for r in set(rates.tolist())}
+    lmax = int(resampled_length(lens, [ratio[r][0] for r in rates.tolist()], [ratio[r][1] for r in rates.tolist()]).max()) \
+        if n else 0
     grp = None
     if world > 1:
         grp = group if group is not None else dist.group.WORLD       # MFCC's call-wide clamp maximum spans the ranks
-    local = predictor._embed_waves([mine[i] for i in range(lo, hi)], lmax, masked=True, to_numpy=False, group=grp)
+    own = rates[lo:hi].tolist()
+    resample = {'rates': own} if any(r != target_sr for r in own) else {}
+    local = predictor._embed_waves([mine[i] for i in range(lo, hi)], lmax, masked=True, to_numpy=False, group=grp,
+                                   **resample)
     full = gather_embeddings(local, n, group)
     return full.cpu().numpy() if as_numpy else full

@@ -125,6 +125,42 @@ class Engine:
         _, Zt = scipy.linalg.eigh_tridiagonal(d, e, select='i', select_range=(0, k - 1))
         return lam, self.sym_tridiag_apply_q(A, tau, Zt).cpu().numpy()
 
+    # ---- input conditioning (csrc/condition.cu) ----
+    def _tap_offsets(self, pairs):
+        """Offsets (float64 elements) of the per-phase tap tables of ``pairs`` in the engine's device tap table; a pair
+        seen for the first time is designed on the host (audio.polyphase_taps) and the table uploaded again."""
+        from .audio import polyphase_taps
+        if not hasattr(self, '_taps'):
+            self._taps, self._tap_off, self._taps_dev = [], {}, None
+        new = [p for p in pairs if p not in self._tap_off]
+        for p in new:
+            self._tap_off[p] = sum(t.size for t in self._taps)
+            self._taps.append(polyphase_taps(*p)[0])
+        if new or self._taps_dev is None:
+            self._taps_dev = torch.from_numpy(np.concatenate(self._taps) if self._taps else np.zeros(1)).to(self.device)
+        return self._tap_off
+
+    def condition_plan(self, n_in, rates, target_rate, target_db=None, max_gain_db=300.0):
+        """Host plan of one conditioning call over rows with ``n_in`` native samples at ``rates`` (ConditionPlan)."""
+        return ConditionPlan(self, n_in, rates, target_rate, target_db, max_gain_db)
+
+    def condition(self, wave, n_in, rates, target_rate, target_db=None, max_gain_db=300.0):
+        """_load_audio's resample + dB normalisation of a device batch: ``wave`` CUDA float32 [B, in_ld], row b holding
+        ``n_in[b]`` samples at ``rates[b]`` Hz.  Rows are resampled to ``target_rate`` where the rate differs
+        (vp_resample, bit-identical to AudioSegment.resample), then normalised to ``target_db`` when it is given
+        (vp_gain_normalize).  -> (y [B, max n_out] zero padded, n_out int64 numpy [B], flags device int32 [B] or None:
+        1 where the gain exceeds ``max_gain_db``; ``ConditionPlan.check`` raises AudioSegment.normalize's ValueError)."""
+        assert wave.is_cuda and wave.dtype == torch.float32 and wave.dim() == 2 and wave.is_contiguous()
+        plan = self.condition_plan(n_in, rates, target_rate, target_db, max_gain_db)
+        B = wave.shape[0]
+        if plan.resample:
+            y = torch.empty(B, max(int(plan.n_out.max()), 1), dtype=torch.float32, device=self.device)
+        else:
+            y = wave.clone()
+        flags = torch.empty(B, dtype=torch.int32, device=self.device) if plan.gain else None
+        plan.run(wave, wave.shape[1], y, y.shape[1], 0, B, flags, plan.scratch(B, y.shape[1]))
+        return y, plan.n_out, flags
+
     # ---- verification metrics (csrc/verify.cu) ----
     def verify(self, scores, labels=None, trial_labels=None, enroll_labels=None, p_target=0.01, c_miss=1, c_fa=1,
                sorted_out=False):
@@ -179,6 +215,90 @@ class Engine:
             self.close()
         except Exception:
             pass
+
+
+class ConditionPlan:
+    """Host plan of one conditioning call: per-row (up, down), output lengths and tap offsets, uploaded to the device
+    ONCE (one small copy before any kernel of the call is enqueued); ``run`` then conditions any row range [lo, hi) with
+    pointer offsets into it, so a staging loop enqueues no further copy."""
+
+    def __init__(self, engine, n_in, rates, target_rate, target_db=None, max_gain_db=300.0):
+        from .audio import resample_ratio, resampled_length
+        self.engine = engine
+        self.target_rate = int(target_rate)
+        self.target_db, self.max_gain_db = target_db, float(max_gain_db)
+        self.n_in = np.asarray(n_in, dtype=np.int64).reshape(-1)
+        B = self.n_in.size
+        self.rates = np.broadcast_to(np.asarray(rates, dtype=np.int64), (B,))
+        ratio = {r: resample_ratio(r, target_rate) for r in set(self.rates.tolist())}
+        self.up = np.fromiter((ratio[r][0] for r in self.rates.tolist()), dtype=np.int32, count=B)
+        self.down = np.fromiter((ratio[r][1] for r in self.rates.tolist()), dtype=np.int32, count=B)
+        self.n_out = resampled_length(self.n_in, self.up, self.down)
+        self.rs_rows = self.up != self.down
+        self.resample = bool(self.rs_rows.any())
+        self.gain = target_db is not None
+        self._meta = None
+        if not (self.resample or self.gain):
+            return
+        tap_off = np.zeros(B, dtype=np.int64)
+        if self.resample:
+            offs = engine._tap_offsets(sorted({p for p, rs in zip(zip(self.up.tolist(), self.down.tolist()), self.rs_rows)
+                                               if rs}))
+            tap_off = np.fromiter((offs.get(p, 0) for p in zip(self.up.tolist(), self.down.tolist())), dtype=np.int64,
+                                  count=B)
+        # one buffer: n_in, n_out, tap_off (int64 [B] each), up, down (int32 [B] each)
+        buf = np.concatenate([self.n_in.view(np.uint8), self.n_out.view(np.uint8), tap_off.view(np.uint8),
+                              self.up.view(np.uint8), self.down.view(np.uint8)])
+        self._meta = torch.from_numpy(buf).to(engine.device)
+        self._base = self._meta.data_ptr()
+        self._B = B
+
+    def rows_resampled(self, lo, hi):
+        return bool(self.rs_rows[lo:hi].any())
+
+    def scratch(self, rows, ld):
+        """Device scratch of the gain for ``rows`` rows of leading dimension ``ld`` (None without gain)."""
+        if not self.gain:
+            return None
+        nb = int(L.lib().vp_gain_scratch_bytes(self.engine.handle, rows, ld))
+        return torch.empty(max(nb, 1), dtype=torch.uint8, device=self.engine.device)
+
+    def _ptr(self, block, itemsize, lo):
+        return C.c_void_p(self._base + 8 * self._B * min(block, 3) + 4 * self._B * max(block - 3, 0) + itemsize * lo)
+
+    def run(self, x, in_ld, y, out_ld, lo, hi, flags, scratch, stream=None):
+        """Condition rows lo..hi: ``x`` native rows [hi - lo, in_ld] -> ``y`` [hi - lo, out_ld] (device float32; with
+        nothing to resample in the range ``y`` must already hold the rows, x is not read), then the gain in place on
+        ``y`` with the rows' flags written to ``flags[lo:hi]`` (a device int32 tensor over ALL rows of the plan)."""
+        eng = self.engine
+        sp = eng.stream_ptr() if stream is None else C.c_void_p(stream.cuda_stream)
+        n = hi - lo
+        if n <= 0:
+            return
+        if self.rows_resampled(lo, hi):
+            _check(eng.handle, L.lib().vp_resample(
+                eng.handle, C.c_void_p(x.data_ptr()), int(in_ld), C.c_void_p(y.data_ptr()), int(out_ld), n,
+                self._ptr(0, 8, lo), self._ptr(1, 8, lo), self._ptr(3, 4, lo), self._ptr(4, 4, lo), self._ptr(2, 8, lo),
+                C.c_void_p(eng._taps_dev.data_ptr()), sp))
+        if self.gain:
+            _check(eng.handle, L.lib().vp_gain_normalize(
+                eng.handle, C.c_void_p(y.data_ptr()), int(out_ld), n, self._ptr(1, 8, lo), float(self.target_db),
+                self.max_gain_db, C.c_void_p(flags.data_ptr() + 4 * lo), C.c_void_p(scratch.data_ptr()), sp))
+
+    def check(self, flags_host, native_rows=None):
+        """Raise AudioSegment.normalize's ValueError for the first flagged row.  The message needs the host's gain:
+        it is recomputed from the row's native samples (``native_rows[i]``), resampled and normalised on the host
+        exactly as _load_audio did -- an error path only."""
+        bad = np.flatnonzero(np.asarray(flags_host))
+        if bad.size == 0:
+            return
+        i = int(bad[0])
+        if native_rows is not None:
+            from .audio import AudioSegment
+            seg = AudioSegment(np.asarray(native_rows[i], dtype=np.float32), int(self.rates[i]))
+            seg.resample(self.target_rate)
+            seg.normalize(target_db=self.target_db, max_gain_db=self.max_gain_db)      # raises with the host's message
+        raise ValueError(f'cannot normalise to {self.target_db} dB: the gain of row {i} exceeds {self.max_gain_db} dB')
 
 
 class WeightArena:

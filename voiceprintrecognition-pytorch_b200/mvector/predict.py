@@ -130,7 +130,7 @@ class MVectorPredictor:
             seg = self._load_audio(p)
             self.users_name.append(os.path.basename(os.path.dirname(p)))
             self.users_audio_path.append(p)
-            pending.append(seg.samples)
+            pending.append(seg)                       # at its own rate: conditioned on the device by predict_batch
             if len(pending) == bs:
                 feats = self.predict_batch(pending)
                 self.audio_feature = feats if self.audio_feature is None else np.vstack((self.audio_feature, feats))
@@ -160,7 +160,9 @@ class MVectorPredictor:
 
     # ------------------------------------------------------------------ hot path
     def _load_audio(self, audio_data, sample_rate=16000):
-        """predict.py:185-212: type dispatch, min-duration assert, resample, dB normalisation."""
+        """predict.py:185-204: decoding, type dispatch and the min-duration assert on the NATIVE duration -> the
+        AudioSegment at its own rate.  Resampling and dB normalisation (predict.py:205-211) run on the device, in the
+        staging of ``_embed_waves``; ``_condition_host`` is the host form for the callers that need host samples."""
         if isinstance(audio_data, str):
             audio_segment = AudioSegment.from_file(audio_data)
         elif isinstance(audio_data, BufferedReader):
@@ -176,6 +178,12 @@ class MVectorPredictor:
         ds = self.configs.dataset_conf.dataset
         assert audio_segment.duration >= ds.min_duration, \
             f'音频太短，最小应该为{ds.min_duration}s，当前音频为{audio_segment.duration}s'
+        return audio_segment
+
+    def _condition_host(self, audio_segment):
+        """predict.py:205-211 on the host, in place: ``register`` writes the normalised samples to disk and
+        ``speaker_diarization`` runs its VAD on them."""
+        ds = self.configs.dataset_conf.dataset
         if audio_segment.sample_rate != ds.sample_rate:
             audio_segment.resample(ds.sample_rate)
         if ds.use_dB_normalization:
@@ -288,9 +296,15 @@ class MVectorPredictor:
             left -= c
         return out
 
-    def _embed_waves(self, waves, lmax, masked, to_numpy=True, group=None):
-        """waves: list of 1-D float32 arrays (already loaded / resampled / normalised) -> [B, embd_dim] (np.float32, or the
-        device tensor with ``to_numpy=False``).
+    def _embed_waves(self, waves, lmax, masked, to_numpy=True, group=None, rates=None):
+        """waves: list of 1-D float32 arrays, decoded, at ``rates`` Hz (None: all at the model's rate) -> [B, embd_dim]
+        (np.float32, or the device tensor with ``to_numpy=False``).  ``lmax`` is the longest item AFTER resampling.
+
+        Conditioning (predict.py:205-211) runs on the device inside the staging: a stage with rows to resample is
+        gathered at its native length into a native-rate device slot and resampled into the model-rate slot
+        (vp_resample); with ``use_dB_normalization`` the rows are then normalised in place (vp_gain_normalize), before
+        the front-end.  A gain above 300 dB raises ValueError before the call returns.  A call that needs neither
+        enqueues nothing of the two.
 
         Reference semantics (predict.py:244-262): every utterance is zero padded to ``lmax`` (the longest item of the WHOLE
         batch -- the caller's batch, which under ``predict_batch_sharded`` is larger than this rank's list), T and the CMN
@@ -322,9 +336,15 @@ class MVectorPredictor:
         eng = fz.engine
         lib = L.lib()
         F = fz.feature_dim
+        ds_conf = self.configs.dataset_conf.dataset
+        lens = np.fromiter(map(len, waves), dtype=np.int32, count=B)
+        plan = None
+        gain_db = ds_conf.target_dB if ds_conf.use_dB_normalization else None
+        if gain_db is not None or (rates is not None and any(int(r) != ds_conf.sample_rate for r in rates)):
+            plan = eng.condition_plan(lens, ds_conf.sample_rate if rates is None else rates, ds_conf.sample_rate, gain_db)
         keep_all = None
         if masked:
-            lens64 = np.fromiter(map(len, waves), dtype=np.int64, count=B)
+            lens64 = plan.n_out if plan is not None else lens.astype(np.int64)
             # float64 quotient rounded once to float32 == torch.tensor([len / lmax ...], dtype=float32) of predict.py:251-255
             keep_all = fz.keep_frames(torch.from_numpy((lens64 / lmax).astype(np.float32)), T).to(dev)
         emb = torch.empty(B, D, dtype=torch.float32, device=dev)
@@ -335,6 +355,13 @@ class MVectorPredictor:
         nstages = (B + S - 1) // S
         K = min(nstages, 4)                             # device staging slots (the pinned side always has two)
         dwave = torch.empty(K, S * lmax, dtype=torch.float32, device=dev)
+        dnat = flags = gscratch = None
+        if plan is not None:
+            if plan.resample:                            # native-rate slots of the stages that resample
+                dnat = torch.empty(K, S * int(lens.max()), dtype=torch.float32, device=dev)
+            if plan.gain:
+                flags = torch.empty(B, dtype=torch.int32, device=dev)
+                gscratch = plan.scratch(S, lmax)
         scratch = torch.empty(max(int(lib.vp_frontend_scratch_floats(eng.handle, S, lmax)), 1), dtype=torch.float32, device=dev)
         if self._copy_stream is None:
             self._copy_stream = torch.cuda.Stream(device=dev)
@@ -344,7 +371,6 @@ class MVectorPredictor:
         main_ptr = C.c_void_p(main.cuda_stream)
         cs.wait_stream(main)                            # buffers handed out by the allocator may still be in use on main
         ptrs = np.empty(B, dtype=np.uint64)              # filled stage by stage: only stage 0's part is on the critical path
-        lens = np.fromiter(map(len, waves), dtype=np.int32, count=B)
         nthreads = self._gather_threads()
         self._configure_gather(lib)
         mark('host prep done (keep, buffers, pointer table)')
@@ -368,11 +394,14 @@ class MVectorPredictor:
                 pin_ev[ps].synchronize()
             if dev_ev[ds] is not None:
                 cs.wait_event(dev_ev[ds])
-            host = self._pinned_slot(ps, n * lmax)
             dw = dwave[ds]
+            resample = plan is not None and plan.rows_resampled(g0, g1)
+            ld = int(lens[g0:g1].max()) if resample else lmax          # a resampling stage stages its native rows
+            dst = dnat[ds] if resample else dw
+            host = self._pinned_slot(ps, n * ld)
             ptrs[g0:g1] = np.fromiter((w.__array_interface__['data'][0] for w in waves[g0:g1]), dtype=np.uint64, count=n)
-            rc = lib.vp_host_stage_h2d(C.c_void_p(ptrs.ctypes.data + 8 * g0), C.c_void_p(lens.ctypes.data + 4 * g0), n, lmax,
-                                       C.c_void_p(host.data_ptr()), C.c_void_p(dw.data_ptr()), self.COPY_SLICE, nthreads, cs_ptr)
+            rc = lib.vp_host_stage_h2d(C.c_void_p(ptrs.ctypes.data + 8 * g0), C.c_void_p(lens.ctypes.data + 4 * g0), n, ld,
+                                       C.c_void_p(host.data_ptr()), C.c_void_p(dst.data_ptr()), self.COPY_SLICE, nthreads, cs_ptr)
             if rc != L.VP_OK:
                 raise L.VpError(rc, 'vp_host_stage_h2d failed')
             mark(f'stage {gi}: {n} utterances gathered, H2D enqueued')
@@ -381,6 +410,9 @@ class MVectorPredictor:
             pin_ev[ps] = cev
             dmark(f'stage {gi}: H2D done', cs)
             main.wait_event(cev)
+            if plan is not None:
+                plan.run(dst, ld, dw, lmax, g0, g1, flags, gscratch, main)
+                dmark(f'stage {gi}: conditioning done', main)
             kp = C.c_void_p(keep_all.data_ptr() + 4 * g0) if keep_all is not None else C.c_void_p()
             if whole and group is not None:
                 fz.mfcc_sharded(dw, n, lmax, kp, feats, scratch, main, group)
@@ -402,6 +434,8 @@ class MVectorPredictor:
         main.wait_stream(cs)
         mark('all kernels enqueued')
         out = emb.cpu().numpy() if to_numpy else emb
+        if flags is not None:
+            plan.check(flags.cpu().numpy(), waves)      # after the result copy: no extra synchronise
         mark('result on host' if to_numpy else 'returned device tensor')
         return out
 
@@ -445,28 +479,34 @@ class MVectorPredictor:
         """预测一个音频的特征 (predict.py:214-229) -> np.ndarray [embd_dim]"""
         seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
         w = np.ascontiguousarray(seg.samples, dtype=np.float32)
-        return self._embed_waves([w], w.shape[0], masked=False)[0]
+        lmax = int(self._output_lengths([w.shape[0]], [seg.sample_rate])[0])
+        return self._embed_waves([w], lmax, masked=False, rates=[seg.sample_rate])[0]
 
     def predict_batch(self, audios_data, sample_rate=16000, batch_size=32):
         """预测一批音频的特征 (predict.py:231-265) -> np.ndarray [B, embd_dim], order preserved."""
-        waves = self._load_batch(audios_data, sample_rate)
-        lmax = max(w.shape[0] for w in waves)
-        return self._embed_waves(waves, lmax, masked=True)
+        waves, rates = self._load_batch(audios_data, sample_rate)
+        lmax = int(self._output_lengths(list(map(len, waves)), rates).max()) if waves else 0
+        return self._embed_waves(waves, lmax, masked=True, rates=rates)
+
+    def _output_lengths(self, n_in, rates):
+        """Sample counts after resampling to the model's rate (int64 numpy): known on the host before anything runs."""
+        from .audio import resample_ratio, resampled_length
+        tsr = self.configs.dataset_conf.dataset.sample_rate
+        ratio = {r: resample_ratio(r, tsr) for r in set(rates)}
+        return resampled_length(n_in, [ratio[r][0] for r in rates], [ratio[r][1] for r in rates])
 
     def _load_batch(self, audios_data, sample_rate=16000):
-        """predict.py:244-247 for a list: every item through ``_load_audio``.  Raw float32 mono arrays that are already at
-        the model's sample rate, with dB normalisation off, come out of ``_load_audio`` unchanged (predict.py:196-211:
-        from_ndarray, duration assert, no resample, no normalise) -- they are checked in one pass and used in place instead
-        of being wrapped and re-wrapped one by one (a 256-utterance batch spends more time in that loop than the GPU in
-        its front-end)."""
+        """predict.py:244-247 for a list -> (decoded float32 rows at their native rate, the rates).  C-contiguous float32
+        1-D arrays come out of ``_load_audio`` unchanged (predict.py:196-204: from_ndarray, duration assert) -- they are
+        checked in one pass and used in place instead of being wrapped one by one (a 256-utterance batch spends more time
+        in that loop than the GPU in its front-end); resampling and normalisation follow on the device."""
         ds = self.configs.dataset_conf.dataset
-        if sample_rate == ds.sample_rate and not ds.use_dB_normalization and all(
-                type(a) is np.ndarray and a.dtype == np.float32 and a.ndim == 1 and a.flags.c_contiguous for a in audios_data):
+        if all(type(a) is np.ndarray and a.dtype == np.float32 and a.ndim == 1 and a.flags.c_contiguous for a in audios_data):
             shortest = min(a.shape[0] for a in audios_data) if len(audios_data) else 0
             if len(audios_data) == 0 or shortest / float(sample_rate) >= ds.min_duration:
-                return list(audios_data)
-        return [np.ascontiguousarray(self._load_audio(audio_data=a, sample_rate=sample_rate).samples, dtype=np.float32)
-                for a in audios_data]
+                return list(audios_data), [int(sample_rate)] * len(audios_data)
+        segs = [self._load_audio(audio_data=a, sample_rate=sample_rate) for a in audios_data]
+        return [np.ascontiguousarray(s.samples, dtype=np.float32) for s in segs], [s.sample_rate for s in segs]
 
     def contrast(self, audio_data1, audio_data2):
         """声纹对比 (predict.py:267-279) -> cosine similarity"""
@@ -476,7 +516,7 @@ class MVectorPredictor:
 
     def register(self, audio_data, user_name: str, sample_rate=16000):
         """声纹注册 (predict.py:281-309)"""
-        seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
+        seg = self._condition_host(self._load_audio(audio_data=audio_data, sample_rate=sample_rate))
         feature = self.predict(audio_data=seg.samples, sample_rate=seg.sample_rate)
         if self.audio_feature is None:
             self.audio_feature = feature
@@ -524,7 +564,9 @@ class MVectorPredictor:
 
     def speaker_diarization(self, audio_data, sample_rate=16000, speaker_num=None, search_audio_db=False):
         """说话人日志识别 (predict.py:365-395) -> [{'speaker': id or name, 'start': s, 'end': s}, ...]"""
-        input_data = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
+        input_data = self._condition_host(self._load_audio(audio_data=audio_data, sample_rate=sample_rate))
+        # the 16 kHz chunks go to predict_batch with the caller's sample_rate, as in the reference (predict.py:379): a
+        # caller at another rate has them resampled a second time
         segments = self.speaker_diarize.segments_audio(input_data)
         features = self.predict_batch([seg[2] for seg in segments], sample_rate=sample_rate)
         labels, spk_center_embeddings = self.speaker_diarize.clustering(features, speaker_num=speaker_num)

@@ -81,13 +81,9 @@ class MVectorTrainer(object):
                         j = j + 1 if j < len(lines) - 1 else 0
                     if seg is None:
                         raise RuntimeError('no usable audio file in ' + data_list)
-                    if seg.sample_rate != sample_rate:
-                        seg.resample(sample_rate)
-                    if use_db:
-                        seg.normalize(target_db=target_db)
-                    if seg.duration > max_duration:
-                        seg.samples = seg.samples[:int(max_duration * seg.sample_rate)]
-                    feature = self.audio_featurizer(torch.from_numpy(seg.samples)).squeeze(0).cpu().numpy()
+                    wave = self._condition(seg, sample_rate, target_db if use_db else None, max_duration,
+                                           self.audio_featurizer.engine)
+                    feature = self.audio_featurizer(wave).squeeze(0).cpu().numpy()
                     label = int(label)
                     stamp = int(time.time() * 1000)
                     save_path = os.path.join(save_dir, str(label), f'{stamp}.npy').replace('\\', '/')
@@ -141,13 +137,36 @@ class MVectorTrainer(object):
             max_feature_len = self.audio_featurizer.num_frames(int(max_duration * sample_rate))
             return torch.from_numpy(np.asarray(np.load(path)[:max_feature_len], dtype=np.float32)).to(self._device)
         seg = AudioSegment.from_file(path)
-        if seg.sample_rate != sample_rate:
-            seg.resample(sample_rate)
-        if use_db:
-            seg.normalize(target_db=target_db)
-        if seg.duration > max_duration:                                          # crop(mode='eval'): from the start
-            seg.samples = seg.samples[:int(max_duration * seg.sample_rate)]
-        return self.audio_featurizer(torch.from_numpy(seg.samples)).squeeze(0)
+        return self.audio_featurizer(self._condition(seg, sample_rate, target_db if use_db else None, max_duration,
+                                                     getattr(self, '_engine', None))).squeeze(0)
+
+    @staticmethod
+    def _condition(seg, sample_rate, target_db, max_duration, eng):
+        """reader.py:82-107 for one decoded file: resample the WHOLE file to ``sample_rate`` and dB-normalise it
+        (``target_db`` not None) on the device of ``eng``, then crop it to ``max_duration`` from the start -> [n] device
+        float32 (Engine.condition; a file already at the rate with normalisation off is uploaded as it is).
+        ``eng`` None is a trainer without a device engine -- the host-logic tests drive evaluate with CPU oracle
+        stand-ins for the featurizer and backbone -- which conditions with AudioSegment on the host (CPU tensor)."""
+        if eng is None:
+            if seg.sample_rate != sample_rate:
+                seg.resample(sample_rate)
+            if target_db is not None:
+                seg.normalize(target_db=target_db)
+            n = seg.samples.shape[0]
+            crop = int(max_duration * sample_rate) if n / float(sample_rate) > max_duration else n
+            return torch.from_numpy(seg.samples[:crop])
+        x = torch.from_numpy(np.ascontiguousarray(seg.samples, dtype=np.float32)).to(eng.device)
+        n = x.shape[0]
+        if seg.sample_rate != sample_rate or target_db is not None:
+            y, n_out, flags = eng.condition(x.unsqueeze(0), [n], [seg.sample_rate], sample_rate, target_db)
+            if flags is not None and int(flags.cpu()[0]):
+                seg.resample(sample_rate)
+                seg.normalize(target_db=target_db)            # raises AudioSegment.normalize's ValueError
+            n = int(n_out[0])
+            x = y[0]
+        if n / float(sample_rate) > max_duration:             # crop(mode='eval'): from the start
+            n = int(max_duration * sample_rate)
+        return x[:n]
 
     def _embed_list(self, data_list):
         """Embeddings of one list in eval order, one eval_conf.batch_size batch at a time: decode -> featurize singly ->
