@@ -5,8 +5,10 @@
 
 Loads the base checkout's package and library, and this tree's, in turn (one process each, VPB_LIB naming the library,
 alternating for --rounds rounds) on the same seeded 256 x 3 s batch: checks that Fbank-80, MelSpectrogram-64,
-Spectrogram-400 and MFCC features are bit-identical between the two, and times vp_fbank at that shape with CUDA events after a warm-up.  Then times every
-framing option of this tree's library at the same shape.  Prints the card's name and power limit with the numbers.
+Spectrogram-400 and MFCC features are bit-identical between the two, and times vp_fbank at that shape with CUDA events after a warm-up,
+and beside it, through AudioFeaturizer, MelSpectrogram-64 (n_fft 1024) at 128 x 5 s and Spectrogram-400 (the mixed-radix
+FFT path) at 256 x 3 s.  Then times every framing option of this tree's library at the 256 x 3 s shape.  Prints the card's
+name and power limit with the numbers.
 """
 import argparse
 import ctypes as C
@@ -82,6 +84,10 @@ def child(root, out, modes):
     res['vp_fbank_ms'] = _time(lambda: _check(h, lib.vp_fbank(h, C.c_void_p(w.data_ptr()), B, N, None,
                                                               C.c_void_p(y.data_ptr()), C.c_void_p(scratch.data_ptr()),
                                                               sp)))
+    w5 = (torch.randn(128, 80000, generator=torch.Generator().manual_seed(1)) * 0.1).cuda()
+    mel, spec = AudioFeaturizer('MelSpectrogram', method_args=CONFIGS[1][1]), AudioFeaturizer('Spectrogram', method_args={})
+    res['beside_ms'] = {'MelSpectrogram-64 n_fft 1024, 128 x 80000': _time(lambda: mel(w5)),
+                        'Spectrogram n_fft 400, 256 x 48000': _time(lambda: spec(w))}
     if modes:
         res['modes'] = []
         for method, args in MODES:
@@ -108,6 +114,7 @@ def main():
     tmp = a.out or tempfile.mkdtemp()
     os.makedirs(tmp, exist_ok=True)
     times = {k: [] for k in roots}
+    beside = {k: {} for k in roots}
     modes = None
     for r in range(a.rounds):
         for k, root in roots.items():
@@ -120,6 +127,8 @@ def main():
                 res = json.load(fh)
             assert os.path.samefile(res['lib'], path) and res['package'].startswith(root + os.sep), res
             times[k].append(res['vp_fbank_ms'])
+            for name, t in res['beside_ms'].items():
+                beside[k].setdefault(name, []).append(t)
             modes = res.get('modes', modes)
     fa, fb = np.load(os.path.join(tmp, 'base0.npz')), np.load(os.path.join(tmp, 'this0.npz'))
     power = subprocess.run(['nvidia-smi', '--query-gpu=power.limit', '--format=csv,noheader', '-i', '0'],
@@ -131,6 +140,9 @@ def main():
         assert same, method
     for k in roots:
         print(f'vp_fbank {B} x {N} samples, {k:4s}: ' + ', '.join(f'{t:.3f}' for t in times[k]) + ' ms')
+    for k in roots:
+        for name, ts in beside[k].items():
+            print(f'{name}, {k:4s}: ' + ', '.join(f'{t:.3f}' for t in ts) + ' ms')
     for method, args, t in modes:
         print(f'{t:8.3f} ms  {method} {args}')
 

@@ -33,7 +33,8 @@ struct vp_handle {
   int* d_mel_start = nullptr;
   int* d_mel_count = nullptr;
   int* d_mel_off = nullptr;
-  float* d_mel_w = nullptr;
+  double* d_mel_w = nullptr;   // the bank's weights widened to fp64, as the mel accumulation consumes them
+  int mel_nw = 0;
   float* d_dct = nullptr;
 };
 
@@ -163,17 +164,21 @@ int vp_frontend_set(vp_handle* h, const vp_frontend_desc* d, const float* window
   }
   const int F = d->n_mels;
   CUDA_TRY(h, cudaMalloc(&h->d_window, sizeof(float) * d->win_length));
-  CUDA_TRY(h, cudaMalloc(&h->d_twiddle, sizeof(double2) * N));
+  std::vector<double2> twx(N + 8);
+  frontend_twiddle_table(N, tw.data(), twx.data());
+  std::vector<double> mel_wd(mel_w, mel_w + (n_w > 0 ? n_w : 0));
+  CUDA_TRY(h, cudaMalloc(&h->d_twiddle, sizeof(double2) * (N + 8)));
   CUDA_TRY(h, cudaMalloc(&h->d_mel_start, sizeof(int) * F));
   CUDA_TRY(h, cudaMalloc(&h->d_mel_count, sizeof(int) * F));
   CUDA_TRY(h, cudaMalloc(&h->d_mel_off, sizeof(int) * F));
-  CUDA_TRY(h, cudaMalloc(&h->d_mel_w, sizeof(float) * (n_w > 0 ? n_w : 1)));
+  CUDA_TRY(h, cudaMalloc(&h->d_mel_w, sizeof(double) * (n_w > 0 ? n_w : 1)));
   CUDA_TRY(h, cudaMemcpy(h->d_window, window, sizeof(float) * d->win_length, cudaMemcpyHostToDevice));
-  CUDA_TRY(h, cudaMemcpy(h->d_twiddle, tw.data(), sizeof(double2) * N, cudaMemcpyHostToDevice));
+  CUDA_TRY(h, cudaMemcpy(h->d_twiddle, twx.data(), sizeof(double2) * (N + 8), cudaMemcpyHostToDevice));
   CUDA_TRY(h, cudaMemcpy(h->d_mel_start, mel_start, sizeof(int) * F, cudaMemcpyHostToDevice));
   CUDA_TRY(h, cudaMemcpy(h->d_mel_count, mel_count, sizeof(int) * F, cudaMemcpyHostToDevice));
   CUDA_TRY(h, cudaMemcpy(h->d_mel_off, mel_off, sizeof(int) * F, cudaMemcpyHostToDevice));
-  if (n_w > 0) CUDA_TRY(h, cudaMemcpy(h->d_mel_w, mel_w, sizeof(float) * n_w, cudaMemcpyHostToDevice));
+  if (n_w > 0) CUDA_TRY(h, cudaMemcpy(h->d_mel_w, mel_wd.data(), sizeof(double) * n_w, cudaMemcpyHostToDevice));
+  h->mel_nw = n_w > 0 ? n_w : 0;
   if (d->post == 1) {
     CUDA_TRY(h, cudaMalloc(&h->d_dct, sizeof(float) * F * d->n_out));
     CUDA_TRY(h, cudaMemcpy(h->d_dct, dct, sizeof(float) * F * d->n_out, cudaMemcpyHostToDevice));
@@ -260,6 +265,7 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
   p.wave = wave; p.feats = feats; p.partial = scratch;
   p.window = h->d_window; p.twiddle = h->d_twiddle;
   p.mel_start = h->d_mel_start; p.mel_count = h->d_mel_count; p.mel_off = h->d_mel_off; p.mel_w = h->d_mel_w;
+  p.mel_nw = h->mel_nw;
   p.B = B; p.L = L; p.T = T; p.kind = h->fe.kind; p.N = h->fe.n_fft; p.WL = h->fe.win_length; p.hop = h->fe.hop;
   p.F = h->fe.n_mels; p.remove_dc = h->fe.remove_dc; p.power = h->fe.power; p.use_log = h->fe.use_log;
   p.fpb = FPB; p.nblk = (T + FPB - 1) / FPB;
@@ -267,12 +273,12 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
   p.pad = p.kind == 0 ? p.WL / 2 - p.hop / 2 : h->fe_opt.pad;
   p.spec_mult = h->fe.power == 2 ? h->fe_opt.spec_scale * h->fe_opt.spec_scale : h->fe_opt.spec_scale;
   p.preemph = h->fe.preemph; p.log_floor = h->fe.log_floor; p.db_mult = h->fe.db_mult; p.cta_max = nullptr;
-  frontend_plan(p);
   if (h->fe.post == 1) {
     MfccParams m;
     float* cta_max = scratch + round4((size_t)B * p.nblk * h->fe.n_out);
     float* mel = cta_max + round4((size_t)B * p.nblk);
     p.feats = mel; p.partial = nullptr; p.cta_max = cta_max;
+    frontend_plan(p);
     m.mel = mel; m.cta_max = cta_max; m.dct = h->d_dct; m.feats = feats; m.partial = scratch;
     m.B = B; m.T = T; m.M = h->fe.n_mels; m.K = h->fe.n_out; m.fpb = FPB; m.nblk = p.nblk; m.n_max = B * p.nblk;
     m.top_db = h->fe.top_db;
@@ -286,6 +292,7 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
     }
     return VP_OK;
   }
+  frontend_plan(p);
   CUDA_TRY(h, launch_frontend(p, keep, st));
   return VP_OK;
 }

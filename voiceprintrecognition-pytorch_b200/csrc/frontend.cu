@@ -9,10 +9,31 @@
 // The same kernel serves torchaudio.transforms.Spectrogram (identity "mel" bank, featurizer.py:43-44) and the mel stage
 // of torchaudio.transforms.MFCC (featurizer.py:45-46), whose AmplitudeToDB / top_db clamp / DCT-II run in mfcc_post_kernel.
 //
-// FFT: two real frames are packed into one complex length-N Stockham autosort FFT held in shared memory.
-// N = 2^a 3^b 5^c (4 | N): radix-8 passes first, then radix 4 / 2, then generic radix-5 / radix-3 passes (torchaudio's
-// default n_fft = 400 = 8*2*5*5); the pass plan comes from the host.  A group of G threads (a multiple of 32, G ~ N/8)
-// owns one FFT and synchronises on its own named barrier, 256/G groups per CTA run independently.
+// FFT: two real frames are packed into one complex length-N Stockham autosort FFT.  N = 2^a 3^b 5^c (4 | N): radix-8
+// passes first, then radix 4 / 2, then generic radix-5 / radix-3 passes (torchaudio's default n_fft = 400 = 8*2*5*5);
+// the pass plan comes from the host.  A group of G threads (a multiple of 32, G ~ N/8) owns one FFT and synchronises on
+// its own named barrier, 256/G groups per CTA run independently.
+//
+// N = 256 / 512 / 1024 / 2048 (every shipped config) run frontend_kernel<N>: a thread holds its 8 points in registers
+// through every pass (one radix-8 butterfly, or two radix-4 / four radix-2 ones), the window stage produces the first
+// pass's operands in place, and the packed-spectrum split + power reads its own bins from the registers of the last
+// pass and only the mirrored bins Z[N-k] from shared memory.  Any other N runs frontend_kernel<0>, the same arithmetic
+// driven by the pass plan with every operand going through shared memory.  Both use the layouts below.
+//
+// SHARED-MEMORY LAYOUTS (16-byte double2 accesses are served a quarter-warp at a time: 8 lanes x 16 B = all 32 banks,
+// so an access is conflict-free when its 8 lanes hit 8 different 16-byte slots mod 8, or the same slot).
+//  * Exchange between passes: element i lives at slot xpad(i) = i + i/8.  A pass reads src[j + r*q] with j = the lane:
+//    8 consecutive j (q a multiple of 8 for every power-of-two N) share j/8, so they hit 8 consecutive slots.  A pass
+//    writes dst[(j-kk)*R + kk + m*Ns], kk = j % Ns.  Ns = 1 (first pass, R = 8): slot 9j + m, stride 9 over the lanes.
+//    Ns >= 8 (8, 64, 512; 16, 40, 80, ... in the mixed-radix plans, all multiples of 8): the 8 lanes have consecutive
+//    kk and share (j-kk) and i/8, so again 8 consecutive slots.  The unpadded layout had the Ns = 1 stores 8-way
+//    conflicting.  Only the mixed-radix sizes whose q is not a multiple of 8 (n_fft 400: q = 50) keep a 2-way
+//    conflict where a lane group straddles a pad.
+//  * Last exchange of the register-resident path: Z[N/2+1 .. N-1] are stored unpadded and read back as Z[N-k] with
+//    k = the lane: ascending on the store side, descending on the load side, 8 adjacent slots either way.
+//  * Twiddles: twx[(Ns-1) + (r-1)*Ns + kk] = exp(-2 pi i r*kk / (Ns*R)) (built once on the host), the N-1 factors laid out so that
+//    the lanes' kk are adjacent (the plain table was read at stride r*step: up to 8-way).  The radix-5 / radix-3
+//    roots are a separate 8-entry table read at one address by every lane.
 //
 // PRECISION.  The window pipeline runs in fp32 op for op like the reference (those roundings are part of what the
 // reference computes); the FFT, the power spectrum and the mel accumulation run in FP64 and are rounded to fp32 once.
@@ -22,8 +43,12 @@
 // torchaudio's own fp32 result is up to 6.1e-4 (log units) away from the exact value of its own formula, an fp32
 // Stockham up to 4.1e-4, this kernel <= 2e-6.  The distance to the reference is therefore the REFERENCE's rounding
 // error; no fp32 implementation can be closer to it than that without replicating its FFT library bit for bit.
-// Cost: the FFT is shared-memory bound, radix 8 in fp64 moves the same bytes as radix 4 in fp32 did.
-// Bound: the algorithmic traffic is 4*L + 4*T*F bytes per utterance (HBM); the kernel is shared-memory bound (DESIGN.md).
+// Every butterfly, twiddle product, power and mel sum is the same expression on the same operands in both
+// instantiations, so the features do not depend on which one ran.
+// Bound (DESIGN.md section 4 has the counts): at 256 x 3 s, 73 MB of HBM traffic, ~1 GFLOP of fp64 and ~3.2 GB through
+// shared memory per call.  frontend_kernel<512> takes 0.285 ms there and vp_fbank, with cmn_mask_kernel, 0.307 ms (one
+// H100 80GB HBM3, 700 W; vp_fbank took 0.61 ms before the layouts above): shared memory is the nearest bound, ~3x
+// away; the rest is barrier and shared-memory latency at the 16 warps per SM that 128 registers allow.
 #include "kernels.cuh"
 
 namespace vpb {
@@ -37,37 +62,155 @@ __device__ __forceinline__ cd cmi(cd a) { return {a.y, -a.x}; }                 
 __device__ __forceinline__ cd ld2(const double2* p) { const double2 v = *p; return {v.x, v.y}; }
 __device__ __forceinline__ void st2(double2* p, cd v) { *p = make_double2(v.x, v.y); }
 
+// slot of element i in an exchange buffer (header comment: SHARED-MEMORY LAYOUTS)
+__device__ __forceinline__ int xpad(int i) { return i + (i >> 3); }
+static int xpad_len(int N) { return N + (N >> 3); }
+
+// asynchronous global -> shared copy of BYTES (4, 8 or 16, both addresses aligned to it); cp_async_wait_all before use
+template <int BYTES>
+__device__ __forceinline__ void cp_async(void* dst, const void* src) {
+  const unsigned d = (unsigned)__cvta_generic_to_shared(dst);
+  if (BYTES == 16) asm volatile("cp.async.cg.shared.global [%0], [%1], 16;" ::"r"(d), "l"(src) : "memory");
+  else asm volatile("cp.async.ca.shared.global [%0], [%1], %2;" ::"r"(d), "l"(src), "n"(BYTES) : "memory");
+}
+__device__ __forceinline__ void cp_async_wait_all() { asm volatile("cp.async.wait_all;" ::: "memory"); }
+
 // barrier over the G threads of one FFT group (G % 32 == 0; ids 1..8, id 0 is __syncthreads)
 __device__ __forceinline__ void group_sync(int g, int G) { asm volatile("bar.sync %0, %1;" ::"r"(g + 1), "r"(G) : "memory"); }
 
-__global__ void __launch_bounds__(256) frontend_kernel(const __grid_constant__ FrontendParams p) {
-  pdl_launch_dependents();
-  pdl_wait();                 // first access to mutable global memory comes after this
-  extern __shared__ __align__(16) unsigned char smem_raw[];
-  const int N = p.N, WL = p.WL, F = p.F;
-  const int G = p.G;                                // threads per FFT (multiple of 32)
-  const int NG = 256 / G;                           // concurrent FFTs per CTA
-  const int span = (p.fpb - 1) * p.hop + WL;
+// ---- butterflies: v = inputs (twiddles applied), o[m] = output m ----
+__device__ __forceinline__ void bfly8(const cd* v, cd* o) {
+  const cd a0 = cadd(v[0], v[4]), a1 = csub(v[0], v[4]), a2 = cadd(v[2], v[6]), a3 = cmi(csub(v[2], v[6]));
+  const cd a4 = cadd(v[1], v[5]), a5 = csub(v[1], v[5]), a6 = cadd(v[3], v[7]), a7 = cmi(csub(v[3], v[7]));
+  const cd b0 = cadd(a0, a2), b2 = csub(a0, a2), b1 = cadd(a1, a3), b3 = csub(a1, a3);
+  const cd b4 = cadd(a4, a6), b6 = cmi(csub(a4, a6));
+  const double h = 0.70710678118654752440;
+  const cd s5 = cadd(a5, a7), d5 = csub(a5, a7);
+  const cd b5 = {h * (s5.x + s5.y), h * (s5.y - s5.x)};          // * (1 - i) / sqrt 2
+  const cd b7 = {h * (d5.y - d5.x), -h * (d5.x + d5.y)};         // * (-1 - i) / sqrt 2
+  o[0] = cadd(b0, b4); o[1] = cadd(b1, b5); o[2] = cadd(b2, b6); o[3] = cadd(b3, b7);
+  o[4] = csub(b0, b4); o[5] = csub(b1, b5); o[6] = csub(b2, b6); o[7] = csub(b3, b7);
+}
+__device__ __forceinline__ void bfly4(const cd* v, cd* o) {
+  const cd a0 = cadd(v[0], v[2]), a1 = csub(v[0], v[2]), a2 = cadd(v[1], v[3]), a3 = cmi(csub(v[1], v[3]));
+  o[0] = cadd(a0, a2); o[1] = cadd(a1, a3); o[2] = csub(a0, a2); o[3] = csub(a1, a3);
+}
+__device__ __forceinline__ void bfly2(const cd* v, cd* o) {
+  o[0] = cadd(v[0], v[1]);
+  o[1] = csub(v[0], v[1]);
+}
+template <int R>
+__device__ __forceinline__ void bfly(const cd* v, cd* o) {
+  if (R == 8) bfly8(v, o);
+  else if (R == 4) bfly4(v, o);
+  else bfly2(v, o);
+}
 
-  double2* tw = reinterpret_cast<double2*>(smem_raw);               // N
-  double2* bufA = tw + N;                                           // NG * N
-  double2* bufB = bufA + (size_t)NG * N;                            // NG * N
-  float* stage = reinterpret_cast<float*>(bufB + (size_t)NG * N);   // span floats (rounded up to x4)
+// radix of the pass that starts with `rem` points still to combine: frontend_plan's order for a power of two
+__host__ __device__ constexpr int pow2_radix(int rem) { return rem % 8 == 0 ? 8 : (rem % 4 == 0 ? 4 : 2); }
+__host__ __device__ constexpr int pow2_last_radix(int N) { return pow2_radix(N) == N ? N : pow2_last_radix(N / pow2_radix(N)); }
+__host__ __device__ constexpr int pow2_passes(int N) { return N == 1 ? 0 : 1 + pow2_passes(N / pow2_radix(N)); }
+
+// Passes Ns, Ns*R, ... of the register-resident FFT (N = 8 G; thread t holds 8 points).  On entry with Ns == 1 v holds
+// x[t + r*G]; later passes load their operands from src.  Every pass but the last stores to dst in the padded layout and
+// the buffers swap; the last leaves Z[t + i*G + m*Ns] in v[i*R + m] and stores the upper half unpadded.  Returns the
+// buffer of that last store; the other one is free.
+template <int N, int Ns>
+__device__ __forceinline__ double2* fft_pow2(cd (&v)[8], double2* src, double2* dst, const double2* twx, int t, int g) {
+  constexpr int G = N / 8, R = pow2_radix(N / Ns), q = N / R, nb = 8 / R;
+  constexpr bool last = Ns * R == N;
+  if (Ns > 1) {
+#pragma unroll
+    for (int i = 0; i < nb; ++i)
+#pragma unroll
+      for (int r = 0; r < R; ++r) v[i * R + r] = ld2(src + xpad(t + i * G + r * q));
+  }
+#pragma unroll
+  for (int i = 0; i < nb; ++i) {
+    const int j = t + i * G;
+    const int kk = j & (Ns - 1);
+    if (Ns > 1) {
+#pragma unroll
+      for (int r = 1; r < R; ++r) v[i * R + r] = cmul(v[i * R + r], ld2(twx + (Ns - 1) + (r - 1) * Ns + kk));
+    }
+    cd o[R];
+    bfly<R>(&v[i * R], o);
+    const int base = (j - kk) * R + kk;
+#pragma unroll
+    for (int m = 0; m < R; ++m) {
+      v[i * R + m] = o[m];
+      if (!last) st2(dst + xpad(base + m * Ns), o[m]);
+      else if (i * G + m * Ns >= N / 2) st2(dst + j + m * Ns, o[m]);
+    }
+  }
+  group_sync(g, G);
+  if constexpr (last) return dst;
+  else return fft_pow2<N, Ns * R>(v, dst, src, twx, t, g);
+}
+
+// |a|^2 and |b|^2 (or the magnitudes) of the two real frames packed as z = a + i b, from Z[k] and Z[N-k]
+__device__ __forceinline__ void split_power(const FrontendParams& p, cd z, cd zn, double& pa, double& pb) {
+  const double ar = 0.5 * (z.x + zn.x), ai = 0.5 * (z.y - zn.y);
+  const double br = 0.5 * (z.y + zn.y), bi = -0.5 * (z.x - zn.x);
+  pa = ar * ar + ai * ai;
+  pb = br * br + bi * bi;
+  if (p.power == 1) { pa = sqrt(pa); pb = sqrt(pb); }
+  if (p.spec_mult != 1.0) { pa *= p.spec_mult; pb *= p.spec_mult; }     // `normalized`
+}
+
+// NFFT = 256 / 512 / 1024 / 2048: register-resident passes for that n_fft; NFFT = 0: any n_fft, plan-driven.
+// A CTA owns p.tpc consecutive 16-frame tiles of one utterance and emits one CMN partial sum per tile.
+template <int NFFT>
+__global__ void __launch_bounds__(256, 2) frontend_kernel(const __grid_constant__ FrontendParams p) {
+  pdl_launch_dependents();
+  extern __shared__ __align__(16) unsigned char smem_raw[];
+  const int N = NFFT ? NFFT : p.N, WL = p.WL, F = p.F;
+  const int G = NFFT ? NFFT / 8 : p.G;              // threads per FFT (multiple of 32)
+  const int NG = 256 / G;                           // concurrent FFTs per CTA
+  const int cfr = p.fpb * p.tpc;                    // frames per CTA
+  const int span = (cfr - 1) * p.hop + WL;
+  const int XN = N + (N >> 3);
+
+  double2* twx = reinterpret_cast<double2*>(smem_raw);              // N: per-pass twiddles (N - 1 used)
+  double2* roots = twx + N;                                         // 8: W_5^0..4, W_3^0..2
+  double2* bufs = roots + 8;                                        // NG * 2 * XN: exchange buffers A, B of each group
+  double* melw = reinterpret_cast<double*>(bufs + (size_t)NG * 2 * XN);   // mel_nw doubles (rounded up to x2)
+  float* stage = reinterpret_cast<float*>(melw + ((p.mel_nw + 1) & ~1));  // span floats (rounded up to x4)
   float* win = stage + ((span + 3) & ~3);                           // WL
-  float* means = win + ((WL + 3) & ~3);                             // NG * 2
+  float* fcache = win + ((WL + 3) & ~3);                            // cfr * F when p.cache: the CTA's features
+  int* melidx = reinterpret_cast<int*>(fcache + (p.cache ? (size_t)cfr * F : 0));   // start[F], count[F], off[F]
+  float* means = reinterpret_cast<float*>(melidx + 3 * F);          // NG * 2
   float* red = means + NG * 2;                                      // 8 floats: per-warp maxima (MFCC mel stage)
 
   const int tid = threadIdx.x;
   const int b = blockIdx.y;
-  const int f0 = blockIdx.x * p.fpb;
+  const int f0 = blockIdx.x * cfr;
   const int g = tid / G;
   const int t = tid - g * G;
   float vmax = -INFINITY;
   const float* wv = p.wave + (size_t)b * p.L;
 
-  // ---- stage the waveform span, window and twiddles; the frame mode maps each staged sample to its source ----
+  // ---- stage the twiddles, window, mel bank and waveform span with asynchronous copies, all in flight together: one
+  // global-memory latency per CTA instead of one per table.  The tables are immutable, so their copies start before
+  // pdl_wait and overlap the tail of the kernel before this one. ----
+  for (int i = tid; i < N + 8; i += 256) cp_async<16>(twx + i, p.twiddle + i);          // twx and roots are adjacent
+  for (int i = tid; i < p.mel_nw; i += 256) cp_async<8>(melw + i, p.mel_w + i);
+  for (int i = tid; i < WL; i += 256) cp_async<4>(win + i, p.window + i);
+  for (int i = tid; i < F; i += 256) {
+    cp_async<4>(melidx + i, p.mel_start + i);
+    cp_async<4>(melidx + F + i, p.mel_count + i);
+    cp_async<4>(melidx + 2 * F + i, p.mel_off + i);
+  }
+  pdl_wait();                 // first access to mutable global memory comes after this
+  // the frame mode maps each staged sample to its source
   const int q0 = f0 * p.hop;
-  for (int i = tid; i < span; i += 256) {
+  int i0 = 0;
+  if (p.kind == 0 && p.frame != VP_FRAME_KALDI_REFLECT && (reinterpret_cast<size_t>(wv + q0) & 15) == 0) {
+    const int n4 = min(span, p.L - q0) >> 2;        // staged sample i is x[q0 + i]: 16-byte copies while inside the utterance
+    for (int i = tid; i < n4; i += 256) cp_async<16>(stage + 4 * i, wv + q0 + 4 * i);
+    i0 = n4 * 4;
+  }
+  for (int i = i0 + tid; i < span; i += 256) {
     int s = q0 + i;
     if (p.kind == 1) {                      // torch.stft of x zero-extended by p.pad at both ends: functional.py:112-134
       const int Lp = p.L + 2 * p.pad;
@@ -89,15 +232,15 @@ __global__ void __launch_bounds__(256) frontend_kernel(const __grid_constant__ F
     }
     stage[i] = (s >= 0 && s < p.L) ? __ldg(wv + s) : 0.f;
   }
-  for (int i = tid; i < WL; i += 256) win[i] = __ldg(p.window + i);
-  for (int i = tid; i < N; i += 256) tw[i] = __ldg(p.twiddle + i);
+  cp_async_wait_all();
   __syncthreads();
 
-  // Every group owns the frame pairs g, g + NG, ... of the CTA's tile and runs them start to finish on its own named
+  // Every group owns the frame pairs g, g + NG, ... of the CTA's tiles and runs them start to finish on its own named
   // barrier: the groups never wait for each other inside the loop.
-  const int npairs = p.fpb / 2;
-  double2* src0 = bufA + (size_t)g * N;
-  double2* dst0 = bufB + (size_t)g * N;
+  const int npairs = cfr / 2;
+  double2* bufA = bufs + (size_t)g * 2 * XN;
+  double2* bufB = bufA + XN;
+  const int NB = N / 2 + 1;
   for (int pair = g; pair < npairs; pair += NG) {
     const int fa = f0 + pair * 2;                   // frames packed as real (fa) and imaginary (fa + 1) parts
     const int oa = (fa - f0) * p.hop;
@@ -132,7 +275,7 @@ __global__ void __launch_bounds__(256) frontend_kernel(const __grid_constant__ F
       mb = means[g * 2 + 1];
     }
     // ---- window pipeline in fp32, op for op as kaldi.py:183-204 / torch.stft's window multiply; FFT input in fp64 ----
-    for (int j = t; j < N; j += G) {
+    auto windowed = [&](int j) -> cd {
       float ya = 0.f, yb = 0.f;
       if (j < WL) {
         const int jp = j > 0 ? j - 1 : 0;
@@ -154,137 +297,184 @@ __global__ void __launch_bounds__(256) frontend_kernel(const __grid_constant__ F
           yb = __fmul_rn(x, wj);
         }
       }
-      src0[j] = make_double2((double)ya, (double)yb);
+      return {(double)ya, (double)yb};
+    };
+
+    // P[2][N/2+1]: the two power spectra, in whichever exchange buffer the FFT's last pass did not write
+    double* P;
+    if constexpr (NFFT != 0) {
+      // ---- register-resident FFT: the first store goes to A, so the last lands in A when the pass count is odd ----
+      cd v[8];
+#pragma unroll
+      for (int r = 0; r < 8; ++r) v[r] = windowed(t + r * (NFFT / 8));
+      const double2* zbuf = fft_pow2<NFFT, 1>(v, bufB, bufA, twx, t, g);
+      P = reinterpret_cast<double*>(zbuf == bufA ? bufB : bufA);
+      // ---- split the packed spectrum, power in fp64 (kaldi.py:616-618): Z[k] from the registers, Z[N-k] from zbuf ----
+      constexpr int LR = pow2_last_radix(NFFT), LNs = NFFT / LR;
+#pragma unroll
+      for (int i = 0; i < 8 / LR; ++i)
+#pragma unroll
+        for (int m = 0; m < LR; ++m) {
+          constexpr int Gc = NFFT / 8;
+          const int kb = i * Gc + m * LNs;           // v[i * LR + m] = Z[t + kb]
+          if (kb < NFFT / 2 || (kb == NFFT / 2 && t == 0)) {
+            const int k = t + kb;
+            const cd z = v[i * LR + m];
+            const cd zn = (k == 0 || kb == NFFT / 2) ? z : ld2(zbuf + (NFFT - k));
+            double pa, pb;
+            split_power(p, z, zn, pa, pb);
+            P[k] = pa;
+            P[NB + k] = pb;
+          }
+        }
+    } else {
+      for (int j = t; j < N; j += G) st2(bufA + xpad(j), windowed(j));
+      group_sync(g, G);
+      // ---- Stockham autosort FFT in fp64, pass plan from the host (radix 8 / 4 / 2, then 5 / 3) ----
+      double2* src = bufA;
+      double2* dst = bufB;
+      int Ns = 1;
+      for (int ps = 0; ps < p.n_pass; ++ps) {
+        const int R = p.radix[ps];
+        const int q = N / R;
+        const bool pow2 = (Ns & (Ns - 1)) == 0;
+        for (int j = t; j < q; j += G) {
+          const int kk = pow2 ? (j & (Ns - 1)) : (j % Ns);
+          const int base = (j - kk) * R + kk;
+          const double2* tq = twx + (Ns - 1) + kk - Ns;      // tq[r * Ns] = twiddle[r * kk * N / (Ns * R)]
+          if (R == 8 || R == 4 || R == 2) {
+            cd v[8], o[8];
+#pragma unroll
+            for (int r = 0; r < 8; ++r)
+              if (r < R) {
+                v[r] = ld2(src + xpad(j + r * q));
+                if (r > 0 && Ns > 1) v[r] = cmul(v[r], ld2(tq + r * Ns));
+              }
+            if (R == 8) bfly8(v, o);
+            else if (R == 4) bfly4(v, o);
+            else bfly2(v, o);
+#pragma unroll
+            for (int m = 0; m < 8; ++m)
+              if (m < R) st2(dst + xpad(base + m * Ns), o[m]);
+          } else {
+            // generic odd radix (5 or 3): out[m] = sum_r v[r] * W_R^(r m)
+            const double2* wr = roots + (R == 5 ? 0 : 5);
+            cd v[5];
+#pragma unroll
+            for (int r = 0; r < 5; ++r)
+              if (r < R) {
+                v[r] = ld2(src + xpad(j + r * q));
+                if (r > 0 && Ns > 1) v[r] = cmul(v[r], ld2(tq + r * Ns));
+              }
+#pragma unroll
+            for (int m = 0; m < 5; ++m)
+              if (m < R) {
+                cd acc = v[0];
+#pragma unroll
+                for (int r = 1; r < 5; ++r)
+                  if (r < R) acc = cadd(acc, cmul(v[r], ld2(wr + (r * m) % R)));
+                st2(dst + xpad(base + m * Ns), acc);
+              }
+          }
+        }
+        group_sync(g, G);
+        double2* tmp = src; src = dst; dst = tmp;
+        Ns *= R;
+      }
+      // ---- split the packed spectrum, power in fp64 (kaldi.py:616-618) ----
+      P = reinterpret_cast<double*>(dst);
+      for (int k = t; k < NB; k += G) {
+        double pa, pb;
+        split_power(p, ld2(src + xpad(k)), ld2(src + xpad(k == 0 ? 0 : N - k)), pa, pb);
+        P[k] = pa;
+        P[NB + k] = pb;
+      }
     }
     group_sync(g, G);
 
-    // ---- Stockham autosort FFT in fp64, pass plan from the host (radix 8 / 4 / 2, then 5 / 3) ----
-    double2* src = src0;
-    double2* dst = dst0;
-    int Ns = 1;
-    for (int ps = 0; ps < p.n_pass; ++ps) {
-      const int R = p.radix[ps];
-      const int q = N / R;
-      const int step = q / Ns;                      // N / (Ns * R)
-      const bool pow2 = (Ns & (Ns - 1)) == 0;
-      for (int j = t; j < q; j += G) {
-        const int kk = pow2 ? (j & (Ns - 1)) : (j % Ns);
-        const int base = (j - kk) * R + kk;
-        if (R == 8) {
-          cd v[8];
+    // ---- sparse triangular mel projection (fp64 accumulate, rounded once) + log floor (kaldi.py:630-633): the 2 F
+    // outputs of the frame pair over the G threads ----
+    auto emit = [&](int o, double acc) {            // output o of the pair: frame o / F, bin o % F
+      const int fr = o >= F, m = o - fr * F;
+      float s = (float)acc;
+      if (p.use_log == 1) s = logf(fmaxf(s, p.log_floor));                       // kaldi.py:633
+      else if (p.use_log == 2) s = p.db_mult * log10f(fmaxf(s, p.log_floor));   // amplitude_to_DB, functional.py:389-391
+      else if (p.use_log == 3) s = logf(s + p.log_floor);                        // MFCC(log_mels=True), transforms MFCC.forward
+      vmax = fmaxf(vmax, s);
+      p.feats[((size_t)b * p.T + fa + fr) * F + m] = s;
+      if (p.cache) fcache[(size_t)(fa + fr - f0) * F + m] = s;
+    };
+    // Inside a bin the order i = 0 .. cnt-1 is the result's.  With several outputs per thread (Fbank-80: 160 on 64
+    // threads, short chains) four of them run interleaved; with at most one per thread (64 mel bins at n_fft 1024: long
+    // chains) the plain loop pipelines its loads better, and the plan-driven kernel has no registers to spare for more.
+    constexpr int MU = 4;
+    if (NFFT == 0 || 2 * F <= G) {
+      for (int o = t; o < 2 * F && (o < F || vb); o += G) {
+        const int fr = o >= F, m = o - fr * F;
+        const double* pf = P + fr * NB + melidx[m];
+        const double* wf = melw + melidx[2 * F + m];
+        const int cnt = melidx[F + m];
+        double acc = 0.0;
+        for (int i = 0; i < cnt; ++i) acc = fma(pf[i], wf[i], acc);
+        emit(o, acc);
+      }
+    } else {
+      for (int o0 = t; o0 < 2 * F; o0 += MU * G) {
+        const double* pf[MU];
+        const double* wf[MU];
+        int cnt[MU], cmax = 0;
+        double acc[MU];
 #pragma unroll
-          for (int r = 0; r < 8; ++r) {
-            v[r] = ld2(src + j + r * q);
-            if (r > 0 && Ns > 1) v[r] = cmul(v[r], ld2(tw + r * kk * step));
-          }
-          const cd a0 = cadd(v[0], v[4]), a1 = csub(v[0], v[4]), a2 = cadd(v[2], v[6]), a3 = cmi(csub(v[2], v[6]));
-          const cd a4 = cadd(v[1], v[5]), a5 = csub(v[1], v[5]), a6 = cadd(v[3], v[7]), a7 = cmi(csub(v[3], v[7]));
-          const cd b0 = cadd(a0, a2), b2 = csub(a0, a2), b1 = cadd(a1, a3), b3 = csub(a1, a3);
-          const cd b4 = cadd(a4, a6), b6 = cmi(csub(a4, a6));
-          const double h = 0.70710678118654752440;
-          const cd s5 = cadd(a5, a7), d5 = csub(a5, a7);
-          const cd b5 = {h * (s5.x + s5.y), h * (s5.y - s5.x)};          // * (1 - i) / sqrt 2
-          const cd b7 = {h * (d5.y - d5.x), -h * (d5.x + d5.y)};         // * (-1 - i) / sqrt 2
-          st2(dst + base, cadd(b0, b4));          st2(dst + base + Ns, cadd(b1, b5));
-          st2(dst + base + 2 * Ns, cadd(b2, b6)); st2(dst + base + 3 * Ns, cadd(b3, b7));
-          st2(dst + base + 4 * Ns, csub(b0, b4)); st2(dst + base + 5 * Ns, csub(b1, b5));
-          st2(dst + base + 6 * Ns, csub(b2, b6)); st2(dst + base + 7 * Ns, csub(b3, b7));
-        } else if (R == 4) {
-          cd v0 = ld2(src + j), v1 = ld2(src + j + q), v2 = ld2(src + j + 2 * q), v3 = ld2(src + j + 3 * q);
-          if (Ns > 1) {
-            v1 = cmul(v1, ld2(tw + kk * step));
-            v2 = cmul(v2, ld2(tw + 2 * kk * step));
-            v3 = cmul(v3, ld2(tw + 3 * kk * step));
-          }
-          const cd a0 = cadd(v0, v2), a1 = csub(v0, v2), a2 = cadd(v1, v3), a3 = cmi(csub(v1, v3));
-          st2(dst + base, cadd(a0, a2));          st2(dst + base + Ns, cadd(a1, a3));
-          st2(dst + base + 2 * Ns, csub(a0, a2)); st2(dst + base + 3 * Ns, csub(a1, a3));
-        } else if (R == 2) {
-          const cd v0 = ld2(src + j);
-          cd v1 = ld2(src + j + q);
-          if (Ns > 1) v1 = cmul(v1, ld2(tw + kk * step));
-          st2(dst + base, cadd(v0, v1));
-          st2(dst + base + Ns, csub(v0, v1));
-        } else {
-          // generic odd radix (5 or 3): out[m] = sum_r v[r] * W_R^(r m), W_R^k = tw[k * N / R]
-          cd v[5];
+        for (int u = 0; u < MU; ++u) {
+          const int o = o0 + u * G, fr = o >= F;
+          const bool live = o < 2 * F && (!fr || vb);
+          const int m = live ? o - fr * F : 0;
+          pf[u] = P + fr * NB + melidx[m];
+          wf[u] = melw + melidx[2 * F + m];
+          cnt[u] = live ? melidx[F + m] : 0;
+          cmax = max(cmax, cnt[u]);
+          acc[u] = 0.0;
+        }
+        for (int i = 0; i < cmax; ++i)
 #pragma unroll
-          for (int r = 0; r < 5; ++r)
-            if (r < R) {
-              v[r] = ld2(src + j + r * q);
-              if (r > 0 && Ns > 1) v[r] = cmul(v[r], ld2(tw + r * kk * step));
-            }
+          for (int u = 0; u < MU; ++u)
+            if (i < cnt[u]) acc[u] = fma(pf[u][i], wf[u][i], acc[u]);
 #pragma unroll
-          for (int m = 0; m < 5; ++m)
-            if (m < R) {
-              cd acc = v[0];
-#pragma unroll
-              for (int r = 1; r < 5; ++r)
-                if (r < R) acc = cadd(acc, cmul(v[r], ld2(tw + ((r * m) % R) * q)));
-              st2(dst + base + m * Ns, acc);
-            }
+        for (int u = 0; u < MU; ++u) {
+          const int o = o0 + u * G;
+          if (o < 2 * F && (o < F || vb)) emit(o, acc[u]);
         }
       }
-      group_sync(g, G);
-      double2* tmp = src; src = dst; dst = tmp;
-      Ns *= R;
     }
-
-    // ---- split the packed spectrum, power in fp64 (kaldi.py:616-618) into P[2][N/2+1] (reuses the idle FFT buffer) ----
-    const int NB = N / 2 + 1;
-    double* P = reinterpret_cast<double*>(dst);
-    for (int k = t; k < NB; k += G) {
-      const cd z = ld2(src + k);
-      const cd zn = ld2(src + (k == 0 ? 0 : N - k));
-      const double ar = 0.5 * (z.x + zn.x), ai = 0.5 * (z.y - zn.y);
-      const double br = 0.5 * (z.y + zn.y), bi = -0.5 * (z.x - zn.x);
-      double pa = ar * ar + ai * ai, pb = br * br + bi * bi;
-      if (p.power == 1) { pa = sqrt(pa); pb = sqrt(pb); }
-      if (p.spec_mult != 1.0) { pa *= p.spec_mult; pb *= p.spec_mult; }     // `normalized`
-      P[k] = pa;
-      P[NB + k] = pb;
-    }
-    group_sync(g, G);
-
-    // ---- sparse triangular mel projection (fp64 accumulate, rounded once) + log floor (kaldi.py:630-633) ----
-#pragma unroll
-    for (int fr = 0; fr < 2; ++fr) {
-      if (fr == 1 && !vb) break;
-      const int f = fa + fr;
-      const double* pf = P + fr * NB;
-      for (int m = t; m < F; m += G) {
-        const int st = __ldg(p.mel_start + m), cnt = __ldg(p.mel_count + m), off = __ldg(p.mel_off + m);
-        double acc = 0.0;
-        for (int i = 0; i < cnt; ++i) acc = fma(pf[st + i], (double)__ldg(p.mel_w + off + i), acc);
-        float s = (float)acc;
-        if (p.use_log == 1) s = logf(fmaxf(s, p.log_floor));                       // kaldi.py:633
-        else if (p.use_log == 2) s = p.db_mult * log10f(fmaxf(s, p.log_floor));   // amplitude_to_DB, functional.py:389-391
-        else if (p.use_log == 3) s = logf(s + p.log_floor);                        // MFCC(log_mels=True), transforms MFCC.forward
-        vmax = fmaxf(vmax, s);
-        p.feats[((size_t)b * p.T + f) * F + m] = s;
-      }
-    }
-    group_sync(g, G);                               // P (in the FFT buffer) is overwritten by the next pair
+    // P is in A when the pass count is even, and the next pair's first pass writes A without a barrier before it
+    if (NFFT == 0 || pow2_passes(NFFT ? NFFT : 1) % 2 == 0) group_sync(g, G);
   }
   __syncthreads();
 
+  const int blk0 = blockIdx.x * p.tpc;              // the CTA's first 16-frame tile
   if (p.cta_max) {
-    // ---- MFCC mel stage: per-CTA maximum for the call-wide top_db clamp (functional.py:393-399); CMN comes after the DCT
+    // ---- MFCC mel stage: the CTA's maximum, for every tile it owns, for the call-wide top_db clamp
+    // (functional.py:393-399); CMN comes after the DCT
     vmax = warp_max(vmax);
     if ((tid & 31) == 0) red[tid >> 5] = vmax;
     __syncthreads();
-    if (tid == 0) {
+    if (tid < p.tpc && blk0 + tid < p.nblk) {
       float m = red[0];
       for (int i = 1; i < 8; ++i) m = fmaxf(m, red[i]);
-      p.cta_max[(size_t)b * p.nblk + blockIdx.x] = m;
+      p.cta_max[(size_t)b * p.nblk + blk0 + tid] = m;
     }
     return;
   }
-  // ---- per-CTA column sums for the CMN mean (featurizer.py:79), fixed summation order ----
-  for (int m = tid; m < F; m += 256) {
+  // ---- per-tile column sums for the CMN mean (featurizer.py:79), fixed summation order; from the on-chip copy of the
+  // features when it fits, else from what this CTA wrote ----
+  for (int i = tid; i < p.tpc * F; i += 256) {
+    const int ti = i / F, m = i - ti * F;
+    if (blk0 + ti >= p.nblk) break;
+    const int fb = f0 + ti * p.fpb;
     float s = 0.f;
-    for (int f = f0; f < f0 + p.fpb && f < p.T; ++f) s += p.feats[((size_t)b * p.T + f) * F + m];
-    p.partial[((size_t)b * p.nblk + blockIdx.x) * F + m] = s;
+    for (int f = fb; f < fb + p.fpb && f < p.T; ++f)
+      s += p.cache ? fcache[(size_t)(f - f0) * F + m] : p.feats[((size_t)b * p.T + f) * F + m];
+    p.partial[((size_t)b * p.nblk + blk0 + ti) * F + m] = s;
   }
 }
 
@@ -350,9 +540,15 @@ __global__ void __launch_bounds__(128) cmn_mask_kernel(float* feats, const float
     float s = 0.f;
     for (int i = 0; i < nblk; ++i) s += partial[((size_t)b * nblk + i) * F + m];
     const float mean = s / (float)T;
-    for (int t = t0; t < t0 + rows_per_cta && t < T; ++t) {
-      float* q = feats + ((size_t)b * T + t) * F + m;
-      *q = (t < kp) ? (*q - mean) : 0.f;
+    const int t1 = min(t0 + rows_per_cta, T);
+    for (int tb = t0; tb < t1; tb += 16) {                   // 16 rows in flight: all their loads, then their stores
+      float v[16];
+#pragma unroll
+      for (int u = 0; u < 16; ++u)
+        if (tb + u < t1 && tb + u < kp) v[u] = feats[((size_t)b * T + tb + u) * F + m];
+#pragma unroll
+      for (int u = 0; u < 16; ++u)
+        if (tb + u < t1) feats[((size_t)b * T + tb + u) * F + m] = (tb + u < kp) ? (v[u] - mean) : 0.f;
     }
   }
 }
@@ -384,44 +580,86 @@ static int frontend_group_threads(int N) {
   return G;
 }
 
-// host-side pass plan: radix 8 first, then 4, 2, 5, 3 (N = 2^a 3^b 5^c checked by vp_frontend_set)
-void frontend_plan(FrontendParams& p) {
-  int n = p.N, k = 0;
+// radix 8 first, then 4, 2, 5, 3 (N = 2^a 3^b 5^c checked by vp_frontend_set); returns the number of passes
+static int plan_radices(int N, int* radix) {
+  int n = N, k = 0;
   for (int r : {8, 4, 2, 5, 3})
-    while (n % r == 0 && k < 12) { p.radix[k++] = r; n /= r; }
-  p.n_pass = k;
+    while (n % r == 0 && k < 12) { radix[k++] = r; n /= r; }
+  return k;
+}
+
+// The device twiddle table (FrontendParams::twiddle), N + 8 entries, from tw[k] = exp(-2 pi i k / N): the pass that starts
+// at sub-transform length Ns with radix R owns out[(Ns-1) + (r-1)*Ns + kk] = tw[r * kk * N / (Ns * R)] for r = 1 .. R-1,
+// kk < Ns (adjacent lanes read adjacent entries); out[N-1] is unused; out[N .. N+4] = W_5^k, out[N+5 .. N+7] = W_3^k.
+void frontend_twiddle_table(int N, const double2* tw, double2* out) {
+  int radix[12];
+  const int n_pass = plan_radices(N, radix);
+  int Ns = 1;
+  for (int ps = 0; ps < n_pass; Ns *= radix[ps++])
+    for (int r = 1; r < radix[ps]; ++r)
+      for (int kk = 0; kk < Ns; ++kk) out[(Ns - 1) + (r - 1) * Ns + kk] = tw[r * kk * (N / (Ns * radix[ps]))];
+  out[N - 1] = make_double2(0.0, 0.0);
+  for (int k = 0; k < 8; ++k) {
+    const int R = k < 5 ? 5 : 3, e = k < 5 ? k : k - 5;
+    out[N + k] = (N % R == 0) ? tw[e * (N / R)] : make_double2(0.0, 0.0);
+  }
+}
+
+// dynamic shared memory of one CTA that owns `tpc` 16-frame tiles (frontend_kernel's carve-up)
+static size_t frontend_smem_bytes(const FrontendParams& p, int tpc, bool cache) {
+  const int NG = 256 / p.G;
+  const int cfr = p.fpb * tpc;
+  const int span = (cfr - 1) * p.hop + p.WL;
+  return sizeof(double2) * ((size_t)p.N + 8 + 2 * (size_t)NG * xpad_len(p.N)) + sizeof(double) * ((p.mel_nw + 1) & ~1) +
+         sizeof(float) * (((span + 3) & ~3) + ((p.WL + 3) & ~3) + (cache ? (size_t)cfr * p.F : 0) + 3 * p.F + 2 * NG + 8);
+}
+
+// Host-side plan.  Passes: radix 8 first, then 4, 2, 5, 3 (N = 2^a 3^b 5^c checked by vp_frontend_set).  CTA shape: the
+// kernel is held to 128 registers, i.e. two CTAs of 256 threads per SM, so a CTA takes as many 16-frame tiles (4, 2 or
+// 1: the twiddle / window / mel-bank set-up is paid once per CTA) as leave it within half an SM's shared memory,
+// on-chip copy of its features included.  The large n_fft / hop / bin-count combinations that exceed that run one tile
+// per CTA and drop the on-chip copy if it does not fit the 227 KB a CTA may have.
+void frontend_plan(FrontendParams& p) {
+  p.n_pass = plan_radices(p.N, p.radix);
   p.G = frontend_group_threads(p.N);
+  const size_t half_sm = (228 * 1024 - 2 * 1024) / 2, cta_max = 227 * 1024;
+  const bool want = p.cta_max == nullptr;            // the MFCC mel stage emits maxima, no column sums
+  p.tpc = 1;
+  p.cache = want && frontend_smem_bytes(p, 1, true) <= cta_max;
+  for (int tpc : {4, 2})
+    if (tpc <= p.nblk && frontend_smem_bytes(p, tpc, want) <= half_sm) { p.tpc = tpc; p.cache = want; break; }
 }
 
-size_t frontend_smem_bytes(int N, int WL, int hop, int fpb) {
-  const int G = frontend_group_threads(N);
-  const int NG = 256 / G;
-  const int span = (fpb - 1) * hop + WL;
-  return sizeof(double2) * ((size_t)N + 2 * (size_t)NG * N) + sizeof(float) * (((span + 3) & ~3) + ((WL + 3) & ~3) + 2 * NG + 8 + 4);
-}
-
-// MFCC: mel stage (dB values into p.feats = the temporary mel buffer, maxima into p.cta_max), then clamp + DCT into
-// m.feats and the CMN partial sums, then CMN + mask over the K cepstral coefficients.
 // Dynamic shared memory above 48 KB must be opted into once per kernel; remember the largest request so far.
-static cudaError_t ensure_frontend_smem(size_t smem) {
+template <int NFFT>
+static cudaError_t launch_frontend_kernel_n(const FrontendParams& p, size_t smem, cudaStream_t stream) {
   static PerDeviceSmem once;
   if (once.need(smem)) {
-    cudaError_t e = cudaFuncSetAttribute(frontend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
+    cudaError_t e = cudaFuncSetAttribute(frontend_kernel<NFFT>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem);
     if (e != cudaSuccess) return e;
     once.set(smem);
   }
-  return cudaSuccess;
+  dim3 grid((p.nblk + p.tpc - 1) / p.tpc, p.B);
+  launch_pdl(frontend_kernel<NFFT>, grid, 256, smem, stream, p);
+  return cudaGetLastError();
+}
+
+// the instantiation for p.N: register-resident passes for the power-of-two sizes, the plan-driven kernel for the rest
+static cudaError_t launch_frontend_kernel(const FrontendParams& p, cudaStream_t stream) {
+  const size_t smem = frontend_smem_bytes(p, p.tpc, p.cache);
+  switch (p.N) {
+    case 256: return launch_frontend_kernel_n<256>(p, smem, stream);
+    case 512: return launch_frontend_kernel_n<512>(p, smem, stream);
+    case 1024: return launch_frontend_kernel_n<1024>(p, smem, stream);
+    case 2048: return launch_frontend_kernel_n<2048>(p, smem, stream);
+    default: return launch_frontend_kernel_n<0>(p, smem, stream);
+  }
 }
 
 // MFCC stage 1 only: mel dB values + per-CTA maxima, and their maximum into max_out[0] (device) -- the scalar a sharded
 // call all-reduces (MAX) across ranks before stage 2.
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream) {
-  size_t smem = frontend_smem_bytes(p.N, p.WL, p.hop, p.fpb);
-  cudaError_t e = ensure_frontend_smem(smem);
-  if (e != cudaSuccess) return e;
-  dim3 grid(p.nblk, p.B);
-  launch_pdl(frontend_kernel, grid, 256, smem, stream, p);
-  e = cudaGetLastError();
+  cudaError_t e = launch_frontend_kernel(p, stream);
   if (e != cudaSuccess) return e;
   launch_pdl(max_reduce_kernel, 1, 256, 0, stream, p.cta_max, p.B * p.nblk, max_out);
   return cudaGetLastError();
@@ -447,24 +685,16 @@ cudaError_t launch_frontend_mfcc_finish(const FrontendParams& p, const MfccParam
   return cudaGetLastError();
 }
 
+// MFCC: mel stage (dB values into p.feats = the temporary mel buffer, maxima into p.cta_max), then clamp + DCT into
+// m.feats and the CMN partial sums, then CMN + mask over the K cepstral coefficients.
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream) {
-  size_t smem = frontend_smem_bytes(p.N, p.WL, p.hop, p.fpb);
-  cudaError_t e = ensure_frontend_smem(smem);
-  if (e != cudaSuccess) return e;
-  dim3 grid(p.nblk, p.B);
-  launch_pdl(frontend_kernel, grid, 256, smem, stream, p);
-  e = cudaGetLastError();
+  cudaError_t e = launch_frontend_kernel(p, stream);
   if (e != cudaSuccess) return e;
   return launch_frontend_mfcc_finish(p, m, keep, stream);     // clamps against all B*nblk per-CTA maxima (m.n_max)
 }
 
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream) {
-  size_t smem = frontend_smem_bytes(p.N, p.WL, p.hop, p.fpb);
-  cudaError_t e = ensure_frontend_smem(smem);
-  if (e != cudaSuccess) return e;
-  dim3 grid(p.nblk, p.B);
-  launch_pdl(frontend_kernel, grid, 256, smem, stream, p);
-  e = cudaGetLastError();
+  cudaError_t e = launch_frontend_kernel(p, stream);
   if (e != cudaSuccess) return e;
   const int rows = 64;
   dim3 g2((p.T + rows - 1) / rows, p.B);

@@ -6,8 +6,9 @@ namespace vpb {
 
 struct FrontendParams {
   const float* wave; float* feats; float* partial;
-  const float* window; const double2* twiddle;   // twiddle[k] = exp(-2 pi i k / N) in fp64
-  const int* mel_start; const int* mel_count; const int* mel_off; const float* mel_w;
+  const float* window; const double2* twiddle;   // twiddle: the N + 8 entries of frontend_twiddle_table, in fp64
+  const int* mel_start; const int* mel_count; const int* mel_off; const double* mel_w;   // weights widened to fp64
+  int mel_nw;          // entries of mel_w
   int B, L, T, kind, N, WL, hop, F, remove_dc, power, use_log, fpb, nblk;
   int frame;           // VP_FRAME_* of vp_frontend_options
   int pad;             // kind 0 reflect: samples before x[0] (win/2 - hop/2, may be < 0); kind 1: torchaudio's zero pad
@@ -15,8 +16,10 @@ struct FrontendParams {
   float preemph, log_floor, db_mult;
   float* cta_max;      // non-null: MFCC mel stage (per-CTA maxima instead of CMN partial sums)
   int n_pass, radix[12], G;   // FFT pass plan + threads per FFT group (frontend_plan)
+  int tpc, cache;             // fpb-frame tiles per CTA; 1: the CTA keeps its features in shared memory for the sums
 };
-void frontend_plan(FrontendParams& p);
+void frontend_plan(FrontendParams& p);   // fills the line above; every other field must be set
+void frontend_twiddle_table(int N, const double2* tw, double2* out);
 
 // MFCC tail: mel [B,T,M] dB values -> clamp(max - top_db) -> DCT [M,K] -> feats [B,T,K] + CMN partial sums.
 struct MfccParams {
@@ -82,7 +85,6 @@ cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_finish(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
-size_t frontend_smem_bytes(int N, int WL, int hop, int fpb);
 cudaError_t launch_conv_ffma(const ConvParams& p, cudaStream_t stream);
 cudaError_t launch_conv_c1(const ConvParams& p, cudaStream_t stream);
 cudaError_t launch_colstats(const StatsParams& p, cudaStream_t stream);
