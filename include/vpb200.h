@@ -135,6 +135,15 @@ int vp_mfcc_mel(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, float*
 int vp_mfcc_finish(vp_handle* h, int32_t B, int32_t Lpad, const int32_t* keep_frames, float* feats, float* scratch,
                    const float* max_in, void* stream);
 
+/* Host only (no launch, no device access): how a call on B rows of Lpad samples runs frontend_kernel.  stage: 0 for a
+ * vp_fbank / vp_melspec call, 1 for the mel stage of vp_mfcc (it must match the configured front-end).  info[8] =
+ *   [0] instantiation: the n_fft of the register-resident kernel (256, 512, 1024, 2048), 0 for the plan-driven one
+ *   [1] G, threads per FFT group       [2] tpc, 16-frame tiles per CTA   [3] 1 when the CTA caches its features on chip
+ *   [4] FFT passes                     [5] mel projection: 0 plain loop, 1 four interleaved chains
+ *   [6] nblk, 16-frame tiles per row   [7] grid.x, CTAs per row
+ * VP_ERR_INVALID when the call itself would be refused. */
+int vp_frontend_plan_info(const vp_handle* h, int32_t B, int32_t Lpad, int32_t stage, int32_t* info);
+
 /* ------------------------------------------------------------------------------------------------------------
  * Backbone (seam 2).  The host (Python mirror of the reference's mvector/models modules) lowers a model + a concrete (B, T) to a
  * straight-line program of fused ops over a workspace arena; weights live in one packed arena uploaded once.

@@ -66,7 +66,9 @@ def test_spectrogram_against_fp64_spectrum(n_fft, signal):
         assert np.all(got[b, keep[b]:] == 0)
 
 
-# frames: one, one pair, around one 16-frame tile, around two and four tiles (the CTA sizes), and odd counts beyond
+# frames: one, one pair, around one, two and four 16-frame tiles, and odd counts beyond.  Fbank-80 plans one tile per
+# CTA at every T (frontend_plan: two would not fit half an SM's shared memory), so every case here runs one-tile CTAs;
+# the two- and four-tile CTAs are covered by tests/test_gpu_frontend_edges.py.
 @pytest.mark.parametrize('T', [1, 2, 15, 16, 17, 31, 32, 33, 49, 63, 64, 65, 67, 130])
 def test_fbank_frame_counts(T):
     L = 400 + 160 * (T - 1) + 3

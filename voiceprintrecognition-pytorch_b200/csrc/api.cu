@@ -245,6 +245,33 @@ size_t vp_frontend_scratch_floats(const vp_handle* h, int32_t B, int32_t Lpad) {
   return n;
 }
 
+// The waveform length check of every front-end call: "" when B rows of L samples give at least one frame.
+static const char* frontend_call_error(const vp_handle* h, int B, int L) {
+  if (B < 1) return "empty batch";
+  const char* len_err = frontend_length_error(h, L);
+  if (*len_err) return len_err;
+  return vp_num_frames(h, L) < 1 ? "shorter than one frame" : "";
+}
+
+// The planned FrontendParams of a call on B rows of L samples (frontend_call_error(h, B, L) == ""), buffer pointers
+// left null: the one place the launch shape comes from, for run_frontend and vp_frontend_plan_info alike.
+static FrontendParams frontend_params(const vp_handle* h, int B, int L) {
+  FrontendParams p{};
+  const int T = vp_num_frames(h, L);
+  p.window = h->d_window; p.twiddle = h->d_twiddle;
+  p.mel_start = h->d_mel_start; p.mel_count = h->d_mel_count; p.mel_off = h->d_mel_off; p.mel_w = h->d_mel_w;
+  p.mel_nw = h->mel_nw;
+  p.B = B; p.L = L; p.T = T; p.kind = h->fe.kind; p.N = h->fe.n_fft; p.WL = h->fe.win_length; p.hop = h->fe.hop;
+  p.F = h->fe.n_mels; p.remove_dc = h->fe.remove_dc; p.power = h->fe.power; p.use_log = h->fe.use_log;
+  p.fpb = FPB; p.nblk = (T + FPB - 1) / FPB;
+  p.frame = h->fe_opt.frame_mode;
+  p.pad = p.kind == 0 ? p.WL / 2 - p.hop / 2 : h->fe_opt.pad;
+  p.spec_mult = h->fe.power == 2 ? h->fe_opt.spec_scale * h->fe_opt.spec_scale : h->fe_opt.spec_scale;
+  p.preemph = h->fe.preemph; p.log_floor = h->fe.log_floor; p.db_mult = h->fe.db_mult;
+  frontend_plan(p, h->fe.post == 1);
+  return p;
+}
+
 // want_kind / want_post: -1 = whatever is configured (vp_embed_wave).
 // stage: 0 = the whole front-end; 1 = MFCC mel stage only (maximum -> ext_max[0]); 2 = MFCC clamp/DCT/CMN only, clamping
 // against the externally reduced maximum ext_max[0].
@@ -256,29 +283,17 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
   if (want_post >= 0 && h->fe.post != want_post) return fail(h, VP_ERR_INVALID, "front-end post-stage mismatch (vp_melspec vs vp_mfcc)");
   if ((stage != 2 && !wave) || (stage != 1 && !feats) || !scratch || B < 1) return fail(h, VP_ERR_INVALID, "null/empty argument");
   if (stage != 0 && (h->fe.post != 1 || !ext_max)) return fail(h, VP_ERR_INVALID, "two-stage calls are for the MFCC front-end");
-  const char* len_err = frontend_length_error(h, L);
+  const char* len_err = frontend_call_error(h, B, L);
   if (*len_err) return fail(h, VP_ERR_INVALID, "waveform of %d samples: %s", L, len_err);
-  const int T = vp_num_frames(h, L);
-  if (T < 1) return fail(h, VP_ERR_INVALID, "waveform of %d samples is shorter than one frame (%d)", L, h->fe.win_length);
   CUDA_TRY(h, cudaSetDevice(h->device));
-  FrontendParams p;
+  FrontendParams p = frontend_params(h, B, L);
   p.wave = wave; p.feats = feats; p.partial = scratch;
-  p.window = h->d_window; p.twiddle = h->d_twiddle;
-  p.mel_start = h->d_mel_start; p.mel_count = h->d_mel_count; p.mel_off = h->d_mel_off; p.mel_w = h->d_mel_w;
-  p.mel_nw = h->mel_nw;
-  p.B = B; p.L = L; p.T = T; p.kind = h->fe.kind; p.N = h->fe.n_fft; p.WL = h->fe.win_length; p.hop = h->fe.hop;
-  p.F = h->fe.n_mels; p.remove_dc = h->fe.remove_dc; p.power = h->fe.power; p.use_log = h->fe.use_log;
-  p.fpb = FPB; p.nblk = (T + FPB - 1) / FPB;
-  p.frame = h->fe_opt.frame_mode;
-  p.pad = p.kind == 0 ? p.WL / 2 - p.hop / 2 : h->fe_opt.pad;
-  p.spec_mult = h->fe.power == 2 ? h->fe_opt.spec_scale * h->fe_opt.spec_scale : h->fe_opt.spec_scale;
-  p.preemph = h->fe.preemph; p.log_floor = h->fe.log_floor; p.db_mult = h->fe.db_mult; p.cta_max = nullptr;
+  const int T = p.T;
   if (h->fe.post == 1) {
     MfccParams m;
     float* cta_max = scratch + round4((size_t)B * p.nblk * h->fe.n_out);
     float* mel = cta_max + round4((size_t)B * p.nblk);
     p.feats = mel; p.partial = nullptr; p.cta_max = cta_max;
-    frontend_plan(p);
     m.mel = mel; m.cta_max = cta_max; m.dct = h->d_dct; m.feats = feats; m.partial = scratch;
     m.B = B; m.T = T; m.M = h->fe.n_mels; m.K = h->fe.n_out; m.fpb = FPB; m.nblk = p.nblk; m.n_max = B * p.nblk;
     m.top_db = h->fe.top_db;
@@ -292,8 +307,23 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
     }
     return VP_OK;
   }
-  frontend_plan(p);
   CUDA_TRY(h, launch_frontend(p, keep, st));
+  return VP_OK;
+}
+
+int vp_frontend_plan_info(const vp_handle* h, int32_t B, int32_t Lpad, int32_t stage, int32_t* info) {
+  if (!h || !info) return VP_ERR_INVALID;
+  if (!h->fe_set || stage != h->fe.post || *frontend_call_error(h, B, Lpad)) return VP_ERR_INVALID;
+  const FrontendParams p = frontend_params(h, B, Lpad);
+  const int inst = frontend_instantiation(p.N);
+  info[0] = inst;
+  info[1] = p.G;
+  info[2] = p.tpc;
+  info[3] = p.cache;
+  info[4] = p.n_pass;
+  info[5] = frontend_mel_chains(inst, p.F, p.G) ? 1 : 0;
+  info[6] = p.nblk;
+  info[7] = frontend_grid_x(p);
   return VP_OK;
 }
 

@@ -408,7 +408,7 @@ __global__ void __launch_bounds__(256, 2) frontend_kernel(const __grid_constant_
     // threads, short chains) four of them run interleaved; with at most one per thread (64 mel bins at n_fft 1024: long
     // chains) the plain loop pipelines its loads better, and the plan-driven kernel has no registers to spare for more.
     constexpr int MU = 4;
-    if (NFFT == 0 || 2 * F <= G) {
+    if (!frontend_mel_chains(NFFT, F, G)) {
       for (int o = t; o < 2 * F && (o < F || vb); o += G) {
         const int fr = o >= F, m = o - fr * F;
         const double* pf = P + fr * NB + melidx[m];
@@ -619,11 +619,11 @@ static size_t frontend_smem_bytes(const FrontendParams& p, int tpc, bool cache) 
 // 1: the twiddle / window / mel-bank set-up is paid once per CTA) as leave it within half an SM's shared memory,
 // on-chip copy of its features included.  The large n_fft / hop / bin-count combinations that exceed that run one tile
 // per CTA and drop the on-chip copy if it does not fit the 227 KB a CTA may have.
-void frontend_plan(FrontendParams& p) {
+void frontend_plan(FrontendParams& p, bool mfcc_mel) {
   p.n_pass = plan_radices(p.N, p.radix);
   p.G = frontend_group_threads(p.N);
   const size_t half_sm = (228 * 1024 - 2 * 1024) / 2, cta_max = 227 * 1024;
-  const bool want = p.cta_max == nullptr;            // the MFCC mel stage emits maxima, no column sums
+  const bool want = !mfcc_mel;                       // the MFCC mel stage emits maxima, no column sums
   p.tpc = 1;
   p.cache = want && frontend_smem_bytes(p, 1, true) <= cta_max;
   for (int tpc : {4, 2})
@@ -639,7 +639,7 @@ static cudaError_t launch_frontend_kernel_n(const FrontendParams& p, size_t smem
     if (e != cudaSuccess) return e;
     once.set(smem);
   }
-  dim3 grid((p.nblk + p.tpc - 1) / p.tpc, p.B);
+  dim3 grid(frontend_grid_x(p), p.B);
   launch_pdl(frontend_kernel<NFFT>, grid, 256, smem, stream, p);
   return cudaGetLastError();
 }
@@ -647,7 +647,7 @@ static cudaError_t launch_frontend_kernel_n(const FrontendParams& p, size_t smem
 // the instantiation for p.N: register-resident passes for the power-of-two sizes, the plan-driven kernel for the rest
 static cudaError_t launch_frontend_kernel(const FrontendParams& p, cudaStream_t stream) {
   const size_t smem = frontend_smem_bytes(p, p.tpc, p.cache);
-  switch (p.N) {
+  switch (frontend_instantiation(p.N)) {
     case 256: return launch_frontend_kernel_n<256>(p, smem, stream);
     case 512: return launch_frontend_kernel_n<512>(p, smem, stream);
     case 1024: return launch_frontend_kernel_n<1024>(p, smem, stream);

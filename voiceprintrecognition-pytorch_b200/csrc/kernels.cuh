@@ -18,8 +18,18 @@ struct FrontendParams {
   int n_pass, radix[12], G;   // FFT pass plan + threads per FFT group (frontend_plan)
   int tpc, cache;             // fpb-frame tiles per CTA; 1: the CTA keeps its features in shared memory for the sums
 };
-void frontend_plan(FrontendParams& p);   // fills the line above; every other field must be set
+// fills the line above from the shape fields (no pointer is read); mfcc_mel: the MFCC mel stage (maxima, no CMN sums)
+void frontend_plan(FrontendParams& p, bool mfcc_mel);
 void frontend_twiddle_table(int N, const double2* tw, double2* out);
+// The launch's choices, shared by the launcher, the kernel and vp_frontend_plan_info:
+// frontend_kernel<NFFT> for n_fft N (register-resident for the four power-of-two sizes, 0 = plan-driven) ...
+__host__ __device__ constexpr int frontend_instantiation(int N) {
+  return (N == 256 || N == 512 || N == 1024 || N == 2048) ? N : 0;
+}
+// ... whether its mel projection runs four interleaved chains (else the plain loop over the 2F outputs of a pair) ...
+__host__ __device__ constexpr bool frontend_mel_chains(int nfft, int F, int G) { return nfft != 0 && 2 * F > G; }
+// ... and its CTAs per utterance
+inline int frontend_grid_x(const FrontendParams& p) { return (p.nblk + p.tpc - 1) / p.tpc; }
 
 // MFCC tail: mel [B,T,M] dB values -> clamp(max - top_db) -> DCT [M,K] -> feats [B,T,K] + CMN partial sums.
 struct MfccParams {

@@ -92,6 +92,7 @@ def lib():
         'vp_mfcc': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
         'vp_mfcc_mel': (C.c_int, [vp, f32p, i32, i32, f32p, f32p, vp]),
         'vp_mfcc_finish': (C.c_int, [vp, i32, i32, i32p, f32p, f32p, f32p, vp]),
+        'vp_frontend_plan_info': (C.c_int, [vp, i32, i32, i32, i32p]),
         'vp_weights_load': (C.c_int, [vp, C.c_void_p, sz]),
         'vp_program_create': (C.c_int, [vp, C.POINTER(Op), i32, sz, sz, sz, pp]),
         'vp_program_destroy': (None, [vp]),
@@ -140,7 +141,7 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_feature_dim',
            'vp_weights_load', 'vp_program_create', 'vp_program_destroy', 'vp_embed', 'vp_embed_wave',
            'vp_program_launches', 'vp_program_peek', 'vp_embed_profiled', 'vp_program_op_info', 'vp_host_gather_pad',
-           'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_cosine_scores', 'vp_device_zero',
+           'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_frontend_plan_info', 'vp_cosine_scores', 'vp_device_zero',
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
            'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics',
            'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize']
