@@ -11,6 +11,8 @@ Every case names the kernel it is meant to reach (``kernel``) and, for convs, th
 the GPU tests assert the engine from run_profiled, the CPU tests re-derive the kernel from the lowered op with the
 launchers' own predicates (``kernel_of``, ``tc_schedule``), so a table entry cannot drift into covering something else.
 Never imported by the product."""
+import os
+
 import numpy as np
 
 from mvector import _lib as L
@@ -27,10 +29,11 @@ DEFAULT_POLICY = (1536, 512)                # models/base.py
 # ---------------------------------------------------------------------------------------------------------------
 class _Inputs:
     """Column allocator over the program input [rows, width]: every tensor the program reads from outside is a column
-    window of it, filled after the plan is known."""
+    window of it, filled after the plan is known.  ``derived`` columns are computed from other columns (and the weight
+    blob) after the random fill: the host-materialised operand of a gather twin (see ``_conv``)."""
 
     def __init__(self, width):
-        self.width, self.used, self.rows, self.fills = width, 0, 1, []
+        self.width, self.used, self.rows, self.fills, self.derived = width, 0, 1, [], []
 
     def take(self, rows, C, fill=('normal', 1.0, 0.0), skew=0):
         c = self.used + skew
@@ -106,6 +109,7 @@ def _conv(pb, arena, inp, c, rng, expect, src=None, dst=None):
     in_coff = c.get('in_coff', 0)
     xfill = ('normal', c.get('xscale', 1.0), 0.0)
     src2 = None
+    xcol = ycol = None                                         # input columns holding x / the added second source
     if src is not None:
         pass
     elif c1:
@@ -122,13 +126,27 @@ def _conv(pb, arena, inp, c, rng, expect, src=None, dst=None):
             _copy(pb, inp.take(rows_in, Cin2, fill=xfill), src2, rows_in)
     else:
         src = inp.take(rows_in, Cin, fill=xfill, skew=in_coff)
-        if src2_mode != L.SRC2_NONE:
+        xcol = src.coff
+        if src2_mode != L.SRC2_NONE and c.get('src2_width'):
+            # the second source in an allocation of its own (another row pitch, another first column), filled by a copy
+            y = inp.take(rows_in, Cin2, fill=xfill)
+            ycol = y.coff
+            src2 = pb.alloc(rows_in, c['src2_width']).cols(c.get('src2_coff', 0), Cin2)
+            _copy(pb, y, src2, rows_in)
+        elif src2_mode != L.SRC2_NONE:
             src2 = inp.take(rows_in, Cin2, fill=xfill)
+            ycol = src2.coff
     W = rng.standard_normal((N, K)) / np.sqrt(K)
     w = arena.add('w', W) if c1 else arena.add_conv('w', W)
     bias = arena.add('b', rng.standard_normal(N) * 0.1 * c.get('bias_scale', 1.0)) if c.get('bias') else -1
     post = (arena.add('ps', rng.uniform(0.5, 1.5, N)), arena.add('ph', rng.standard_normal(N) * 0.2)) if c.get('post') else None
-    pre = (arena.add('qs', rng.uniform(0.5, 1.5, cin_tot)), arena.add('qh', rng.standard_normal(cin_tot) * 0.2)) if c.get('pre') else None
+    pre = None
+    if c.get('pre'):
+        # 'pow2': signed power-of-two scales, so x * s is exact and fmaf(x, s, h) == fl32(x * s + h) (see twin())
+        s = (rng.choice([-1.0, 1.0], cin_tot) * 2.0 ** rng.integers(-2, 3, cin_tot) if c['pre'] == 'pow2'
+             else rng.uniform(0.5, 1.5, cin_tot))
+        pre = (arena.add('qs', s), arena.add('qh', rng.standard_normal(cin_tot) * 0.2))
+    pre_relu = bool(pre) and c.get('pre_relu', True)
     res = inp.take(rows_out, N, fill=xfill) if c.get('res') else None
     gate = ubias = None
     if c.get('gate'):
@@ -146,11 +164,18 @@ def _conv(pb, arena, inp, c, rng, expect, src=None, dst=None):
     if c.get('sum'):                     # accumulate-into view: prefilled, acc += y, then copied out next to y
         acc = pb.alloc(rows_out, N)
         _copy(pb, inp.take(rows_out, N), acc, rows_out)
+    if c.get('twin'):
+        # MODE 0 twin of an add / prologue conv: everything above is laid out (and drawn from the rngs) exactly as for
+        # the original, and the op reads one extra input block holding the operand the original's gather computes
+        assert xcol is not None and (pre is not None or src2_mode == L.SRC2_ADD), 'twin of an add / prologue conv'
+        op = inp.take(rows_in, Cin)
+        inp.derived.append(dict(col=op.coff, rows=rows_in, C=Cin, x=xcol, y=ycol, pre=pre, pre_relu=pre_relu))
+        src, src2, src2_mode, pre, pre_relu = op, None, L.SRC2_NONE, None, False
     expect[len(pb.ops)] = ENGINES[engine] if not c1 else 0
     main = len(pb.ops)
     pb.conv(src, dst, w, K, Tin, Tout, Fin=Fin, Fout=Fout, KT=KT, KF=KF, sT=c.get('sT', 1), sF=c.get('sF', 1),
             dT=c.get('dT', 1), dF=1, padT=c.get('padT', 0), padF=c.get('padF', 0),
-            pad_mode=c.get('pad_mode', L.PAD_ZERO), bias=bias, pre=pre, pre_relu=bool(c.get('pre')), post=post,
+            pad_mode=c.get('pad_mode', L.PAD_ZERO), bias=bias, pre=pre, pre_relu=pre_relu, post=post,
             act=c.get('act', L.ACT_NONE), act2=c.get('act2', L.ACT_NONE), res=res, gate=gate, ubias=ubias,
             seg_len=c.get('seg_len'), n_seg=n_seg, src2=src2, src2_mode=src2_mode, sum_into=acc,
             engine=ENGINES[engine], c1=c1)
@@ -279,7 +304,32 @@ def build(case):
     width = max(4, (_build(case, 1 << 16)[2].used + 3) // 4 * 4)
     pb, arena, inp, main, expect, consumer, out_rows, out_cols = _build(case, width)
     X = inp.data(np.random.default_rng(case['seed'] + 7919), case.get('scale', 1.0))
-    return Built(case, pb, arena, X, out_rows, out_cols, main, expect, consumer)
+    b = Built(case, pb, arena, X, out_rows, out_cols, main, expect, consumer)
+    for d in inp.derived:
+        X[:d['rows'], d['col']:d['col'] + d['C']] = _gathered(X, b.blob, d)
+    return b
+
+
+def _gathered(X, blob, d):
+    """The A-operand map an add / prologue gather feeds the MMAs, materialised on the host in the kernels' arithmetic:
+    fl32(x + y) for the add, and fmaf(x, s, h) (then max(., 0) with pre_relu) for the prologue.  With power-of-two s,
+    x * s is exact and fl32(fl64(x * s) + h) is the correctly rounded fp32 sum (53 >= 2 * 24 + 2): exactly fmaf."""
+    rows, C = d['rows'], d['C']
+    x = X[:rows, d['x']:d['x'] + C]
+    if d['pre'] is None:
+        return x + X[:rows, d['y']:d['y'] + C]                                  # float32 + float32: one rounding
+    s, h = (blob[o // 4:o // 4 + C].astype(np.float64) for o in d['pre'])
+    assert np.array_equal(np.abs(s), 2.0 ** np.round(np.log2(np.abs(s)))), 'twin needs power-of-two prologue scales'
+    v = (x.astype(np.float64) * s + h).astype(np.float32)
+    return np.maximum(v, np.float32(0)) if d['pre_relu'] else v
+
+
+def twin(case):
+    """The MODE 0 twin of an add / prologue case: same weights blob, geometry, epilogue, tc_bn / tc_kc and engine, reading
+    the host-materialised operand (``_gathered``) as a plain source.  Its output must equal the original's bit for bit:
+    the tensor-core kernel shares everything after the gather (split, MMA order, epilogue) between the modes, and the FFMA
+    kernel runs one gather (common.cuh gather_a4) whose add / prologue are the same fp32 operations."""
+    return dict(case, twin=True)
 
 
 def with_batch(case, B):
@@ -354,9 +404,11 @@ def tc_schedule(o, engine):
     clamps = (L.ACT_NONE, L.ACT_RELU, L.ACT_HARDTANH20)
     simple = (o.ubias == L.BUF_NONE and o.gate == L.BUF_NONE and o.sum == L.BUF_NONE and o.act in clamps
               and o.act2 in clamps)
-    return dict(bn=bn, m_tiles=m_tiles, n_tiles=n_tiles, tiles=tiles, tiles_per_cta=-(-tiles // grid),
+    tiles_per_cta = -(-tiles // grid)                               # :194 my_tiles of CTA 0, the busiest
+    return dict(bn=bn, m_tiles=m_tiles, n_tiles=n_tiles, tiles=tiles, tiles_per_cta=tiles_per_cta,
                 k_blocks=k_blocks, kc=kc, n_chunks=n_chunks, last_chunk=k_blocks - (n_chunks - 1) * kc,
-                m_tail=M % 128, simple=simple,
+                items=tiles_per_cta * k_blocks,                     # :195 total_items: the producers' (tile, K block) stream
+                k_tail=K % 32, m_tail=M % 128, simple=simple,
                 fast=simple and M % 128 == 0 and o.Cout % bn == 0)     # every tile on the fast epilogue
 
 
@@ -374,6 +426,49 @@ def c1_wide(o):
             and o.Cout in (16, 32, 64) and o.KT * o.KF <= 49 and o.out_ld % 4 == 0 and o.out_coff % 4 == 0)
 
 
+def tc_supported(o):
+    """conv_tc.cu:568-578 (conv_tc_supported) on a lowered op; fill_conv (api.cu:628-648) gives M, N, K and w_tc."""
+    K = o.KT * o.KF * (o.Cin + (o.Cin2 if o.src2_mode == L.SRC2_CONCAT else 0))
+    return (o.w_tc >= 0 and o.B * o.Tout * o.Fout >= 1024 and o.Cout >= 16 and o.Cout % 4 == 0 and K % 4 == 0
+            and o.tc_kc >= 0 and o.tc_kc % 64 == 0 and o.tc_bn == tc_tile_n(o.Cout, o.tc_kc > 0)
+            and not (o.pre_s >= 0 and o.src2_mode != L.SRC2_NONE))
+
+
+def tc16_supported(o):
+    """conv_tc.cu:635-641 (conv_tc16_supported): MODE 0 only, a tracked source (amax slot, PlanBuilder.finalize), Cin,
+    CinTot and K multiples of 8, N >= 128."""
+    cin_tot = o.Cin + (o.Cin2 if o.src2_mode == L.SRC2_CONCAT else 0)
+    return (tc_supported(o) and o.amax_in > 0 and o.pre_s < 0 and o.src2_mode != L.SRC2_ADD and o.Cin % 8 == 0
+            and cin_tot % 8 == 0 and o.KT * o.KF * cin_tot % 8 == 0 and o.Cout >= 128)
+
+
+TC16_ON = not os.environ.get('VPB_TC_F16', '').startswith('0')      # api.cu:79-83 (tc16_enabled)
+
+
+def engine_of(o, pref=None, tc16_on=None):
+    """Engine vp_program_create resolves for a lowered, finalized op (api.cu:559-583): ``pref`` is the requested engine
+    (default: the op's own), ``tc16_on`` whether AUTO may pick the fp16 split (default: VPB_TC_F16 as the library reads
+    it).  0 for ops that are not CONV; ValueError where the library refuses the program (VP_ERR_UNSUPPORTED)."""
+    if o.kind != L.OP_CONV:
+        return 0
+    pref = o.engine if pref is None else pref
+    tc16_on = TC16_ON if tc16_on is None else tc16_on
+    ok = tc_supported(o)
+    ok16 = ok and o.w_tc16_q > 0 and o.tc16_descale > 0 and tc16_supported(o)
+    if (pref == L.ENGINE_TC and not ok) or (pref == L.ENGINE_TC16 and not ok16):
+        raise ValueError('shape / operands not supported by the requested tensor-core engine')
+    if pref == L.ENGINE_TC16 or (pref == L.ENGINE_AUTO and ok16 and tc16_on):
+        return L.ENGINE_TC16
+    if pref == L.ENGINE_TC or (pref == L.ENGINE_AUTO and ok):
+        return L.ENGINE_TC
+    return L.ENGINE_FFMA
+
+
+def _tc_suffix(pre, add):
+    """conv_tc.cu:621-624: the prologue selects conv_tc_kernel<2, ...>, else an added second source <1, ...>, else <0>."""
+    return ',pre' if pre else ',add' if add else ''
+
+
 def kernel_of(o, engine):
     """Name of the kernel a lowered op launches with the given resolved conv engine."""
     if o.kind == L.OP_CONV_C1:
@@ -382,7 +477,7 @@ def kernel_of(o, engine):
         if engine == L.ENGINE_TC16:
             return 'conv_tc<f16>'
         if engine == L.ENGINE_TC:
-            return 'conv_tc<tf32>'
+            return 'conv_tc<tf32%s>' % _tc_suffix(o.pre_s >= 0, o.src2_mode == L.SRC2_ADD)
         if small_m_ok(o):
             return 'linear_small_m'
         # conv_ffma.cu:231-240: BN = 128 above N = 64, 64 above N = 32, else 32
@@ -405,6 +500,25 @@ def kernel_of(o, engine):
     raise ValueError(o.kind)
 
 
+BENCH_T = dict(c2=298, c3=298, c4=251, c5=998)     # frames: 3 s Fbank (25 / 10 ms), 5 s Mel (hop 320, centred), 10 s
+
+
+def bench_model(name):
+    """The bench.py configuration's backbone mirror with its seeded weights (oracle.models.random_state_dict, as
+    bench.save_weights); lowering it needs no GPU."""
+    import bench
+    from oracle import models as om
+    from mvector.models import build_model
+    from mvector.utils.utils import dict_to_object
+    cfg = bench.CONFIGS[name]
+    gain = getattr(om, 'CONDITIONED_GAIN', {}).get(cfg['model'])
+    sd = om.random_state_dict(cfg['model'], cfg['fdim'], seed=0, **(dict(gain=gain) if gain is not None else {}),
+                              **cfg['margs'])
+    model = build_model(cfg['fdim'], dict_to_object({'model_conf': {'model': cfg['model'], 'model_args': cfg['margs']}}))
+    model.load_state_dict(sd)
+    return model, cfg
+
+
 def ew_grid_strides(o):
     """True when the ew / pool2d grid (capped at 132 * 32 CTAs of 256 threads, pool.cu:330-332 / :377-380) is smaller
     than the float4 count, i.e. the grid-stride loop runs more than once."""
@@ -418,7 +532,8 @@ def ew_grid_strides(o):
 def _tc(name, engines, **c):
     """A tensor-core conv case, once per engine ('tc' = split TF32, 'tc16' = fp16 split, 'ffma' = exact reference)."""
     for e in engines:
-        kern = {'tc': 'conv_tc<tf32>', 'tc16': 'conv_tc<f16>',
+        kern = {'tc': 'conv_tc<tf32%s>' % _tc_suffix(c.get('pre'), c.get('src2_mode') == L.SRC2_ADD),
+                'tc16': 'conv_tc<f16>',
                 'ffma': 'conv_ffma<%d>' % (128 if c['N'] > 64 else 64 if c['N'] > 32 else 32)}[e]
         TC_CASES[f'{name}-{e}'] = dict(c, op='conv', engine=e, kernel=kern)
 
@@ -475,9 +590,74 @@ _tc('concat_one_alloc', ('tc', 'tc16'), seed=166, B=4, Tin=300, Cin=64, Cin2=64,
 _tc('out_window', ('ffma', 'tc'), seed=167, B=4, Tin=300, Cin=64, N=64, bias=True, act=L.ACT_RELU, out_coff=32,
     in_coff=4)
 
+# ---- the add (conv_tc_kernel<1, ...>) and BN-ReLU prologue (conv_tc_kernel<2, ...>) gathers ----
+# Both run a 2-deep register pipeline (conv_tc.cu:275, refill :339, publish loop :350-354) with their own slots (:131-132)
+# and publish arithmetic (:322-329).  Every case also runs on the FFMA engine, whose gather_a4 (common.cuh:159-190)
+# computes the same operand, and has a MODE 0 twin (tests/test_gpu_conv_gathers.py).  Prologue scales are signed powers
+# of two (the twin needs x * s exact).
+ADD, PRE = dict(src2_mode=L.SRC2_ADD), dict(pre='pow2')
+_GE = ('tc', 'ffma')
+# M = 2049 (a one-row M tail) and every N tile: BN = 16, then 32 ... 128 with a 12-column tail in the last tile.  The
+# ECAPA Res2 add (K = 192, dilation 2, reflect / zero padding alternating); the CAM++ prologue on a column window of a
+# wider map (in_ld > Cin, in_coff = 8), 1x1 and KT = 3 with zero padding alternating
+for _i, _N in enumerate((16, 20, 36, 52, 68, 84, 100, 116)):
+    _bn = max(16, (_N + 15) // 16 * 16)
+    _tc(f'add_m_tail1_n{_N}', _GE, **ADD, seed=500 + _i, B=3, Tin=683, Cin=64, N=_N, KT=3, dT=2, padT=2,
+        pad_mode=L.PAD_REFLECT if _i % 2 == 0 else L.PAD_ZERO, bias=True, act=L.ACT_RELU, post=True,
+        intent=dict(m_tail=1, bn=_bn))
+    _tc(f'pre_m_tail1_n{_N}', _GE, **PRE, seed=520 + _i, B=3, Tin=683, Cin=64, in_coff=8, N=_N,
+        **(dict(KT=3, padT=1) if _i % 2 else {}), bias=True, act=L.ACT_RELU, post=True, intent=dict(m_tail=1, bn=_bn))
+# accumulation-chunk remainders: the add under ERes2Net's (512, 256) policy on a zero-padded 3x3 map with odd Fin
+# (K = 576: 18 K blocks in chunks of 8, 8, 2); the prologue under the default policy (K = 1600: 16, 16, 16, 2)
+_tc('add_eres_k576_3x3_odd_fin', _GE, **ADD, seed=540, policy=ERES_POLICY, B=2, Tin=40, Fin=21, Cin=64, N=64, KT=3,
+    KF=3, padT=1, padF=1, bias=True, act=L.ACT_HARDTANH20, res=True, intent=dict(chunk_remainder=True))
+_tc('pre_default_k1600', _GE, **PRE, seed=541, B=4, Tin=300, Cin=320, N=128, KT=5, padT=2, bias=True, act=L.ACT_RELU,
+    intent=dict(chunk_remainder=True))
+# 133 tiles on 132 CTAs: exactly one CTA runs a second tile
+_tc('add_tiles_133', _GE, **ADD, seed=542, B=7, Tin=2420, Cin=64, N=128, KT=3, dT=3, padT=3, pad_mode=L.PAD_REFLECT,
+    bias=True, act=L.ACT_RELU, post=True, intent=dict(tiles=133, tiles_per_cta=2))
+_tc('pre_tiles_133', _GE, **PRE, seed=543, B=7, Tin=2420, Cin=128, N=128, bias=True, act=L.ACT_RELU, post=True, res=True,
+    intent=dict(tiles=133, tiles_per_cta=2))
+# 64 x 1056 rows = 528 full tiles, 4 per CTA, every one on the fast epilogue; K = 108 (4 K blocks, a K tail of 12)
+_tc('add_4_tiles_per_cta_k_tail', _GE, **ADD, seed=544, B=64, Tin=1056, Cin=36, N=64, KT=3, dT=4, padT=4,
+    pad_mode=L.PAD_REFLECT, bias=True, act=L.ACT_RELU, post=True, res=True,
+    intent=dict(tiles_per_cta=4, k_tail=12, fast=True))
+_tc('pre_4_tiles_per_cta_k_tail', _GE, **PRE, seed=545, B=64, Tin=1056, Cin=36, N=128, KT=3, padT=1, bias=True,
+    act=L.ACT_RELU, post=True, act2=L.ACT_RELU, intent=dict(tiles_per_cta=4, k_tail=12, fast=True))
+# one K block per tile and 3 tiles per CTA (48 x 1056 rows = 396 tiles): the 2-deep pipeline refills across tiles on
+# every item and ends on an odd item; the general epilogue through a feature (ubias + SiLU, gate + tanh)
+_tc('add_kb1_odd_items_ubias_silu', _GE, **ADD, seed=546, B=48, Tin=1056, Cin=32, N=48, bias=True, ubias=True,
+    act=L.ACT_SILU, intent=dict(k_blocks=1, tiles_per_cta=3, items=3, simple=False))
+_tc('pre_kb1_odd_items_gate_tanh', _GE, **PRE, seed=547, B=48, Tin=1056, Cin=8, N=32, KT=3, padT=1, bias=True,
+    gate=True, act2=L.ACT_TANH, intent=dict(k_blocks=1, k_tail=24, tiles_per_cta=3, items=3, simple=False))
+# add: reflect padding at the smallest map the validator accepts (Tin = dilation + 1), dilations 2, 3, 4 of ECAPA's Res2
+for _d in (2, 3, 4):
+    _tc(f'add_reflect_min_tin_d{_d}', _GE, **ADD, seed=548 + _d, B=1200 // (_d + 1), Tin=_d + 1, Cin=64, N=64, KT=3,
+        dT=_d, padT=_d, pad_mode=L.PAD_REFLECT, bias=True, act=L.ACT_RELU, post=True)
+# add: the second source in an allocation of its own, row pitch 84 and first column 12 (x: the program input, pitch =
+# its width, first column 4), accumulated into a view (general epilogue)
+_tc('add_src2_own_alloc', _GE, **ADD, seed=553, B=4, Tin=300, Cin=64, N=128, KT=3, padT=1, in_coff=4, src2_width=84,
+    src2_coff=12, bias=True, act=L.ACT_RELU, sum=True)
+# prologue: zero padding on a 3x3 map (okmask keeps padded taps at 0, not at relu(h)), reflect padding, no ReLU, and
+# CAM++'s last transit (N = 512, K = 1024, BN affine + ReLU after the conv)
+_tc('pre_3x3_zero_pad', _GE, **PRE, seed=554, B=2, Tin=40, Fin=21, Cin=32, N=32, KT=3, KF=3, padT=1, padF=1, bias=True,
+    act=L.ACT_RELU)
+_tc('pre_reflect_d2', _GE, **PRE, seed=555, B=4, Tin=300, Cin=64, N=64, KT=3, dT=2, padT=2, pad_mode=L.PAD_REFLECT,
+    bias=True, act=L.ACT_RELU, post=True)
+_tc('pre_no_relu_zero_pad', _GE, **PRE, pre_relu=False, seed=556, B=4, Tin=300, Cin=64, N=96, KT=3, padT=1,
+    bias=True, post=True)
+_tc('pre_cam_transit_n512_k1024', _GE, **PRE, seed=557, B=4, Tin=300, Cin=1024, N=512, post=True, act2=L.ACT_RELU)
+GATHER_CASES = {n: c for n, c in TC_CASES.items() if c.get('pre') or c.get('src2_mode') == L.SRC2_ADD}
+
 # position invariance: the rows of the first three utterances must not depend on the batch around them.  At B = 16 the
 # 16000 rows are 125 full tiles (fast epilogue, ~8 tiles per CTA); at B = 3 the last tile is a tail (general path).
+# Variants: the plain source, the added second source, the prologue.
 INVARIANCE = dict(op='conv', seed=170, B=16, Tin=1000, Cin=2048, N=512, bias=True, act=L.ACT_RELU, post=True, res=True)
+INVARIANCE_VARIANTS = {'': {}, 'add': ADD, 'pre': PRE}
+
+
+def invariance(variant, engine, B):
+    return dict(INVARIANCE, **INVARIANCE_VARIANTS[variant], engine=engine, B=B)
 
 FFMA_CASES = {}
 # linear_small_m_kernel: M <= 1024 pointwise linears (SE MLPs, ASP per-utterance bias, final FC)

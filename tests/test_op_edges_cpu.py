@@ -167,8 +167,9 @@ def test_interpreter_matches_torch(name):
 
 
 def test_interpreter_matches_torch_on_position_invariance_case():
-    b = oc.build(oc.with_batch(dict(oc.INVARIANCE, engine='tc'), 1))
-    np.testing.assert_allclose(oc.sim(b), TorchRef(b).run(), rtol=1e-6, atol=1e-9)
+    for variant in oc.INVARIANCE_VARIANTS:
+        b = oc.build(oc.invariance(variant, 'tc', 1))
+        np.testing.assert_allclose(oc.sim(b), TorchRef(b).run(), rtol=1e-6, atol=1e-9)
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -218,10 +219,10 @@ def test_tc_cases_have_the_schedules_they_claim():
 
 
 def test_tc_coverage():
-    """The tables reach the schedules the issue lists: >= 4 tiles per CTA and exactly 133 tiles on both tensor-core
-    engines, a chunk remainder under both chunk policies on both, every N-tile width, M tails of one row and tiles that
-    all take the fast epilogue."""
-    S = _sched()
+    """The plain-source kernels (conv_tc<tf32>, conv_tc<f16>) reach >= 4 tiles per CTA and exactly 133 tiles on both
+    tensor-core engines, a chunk remainder under both chunk policies on both, every N-tile width, M tails of one row and
+    tiles that all take the fast epilogue.  (The add / prologue families: tests/test_conv_gathers_cpu.py.)"""
+    S = {n: (c, s) for n, (c, s) in _sched().items() if c['kernel'] in ('conv_tc<tf32>', 'conv_tc<f16>')}
     for eng in ('tc', 'tc16'):
         mine = {n: s for n, (c, s) in S.items() if c['engine'] == eng}
         assert any(s['tiles_per_cta'] >= 4 for s in mine.values()), eng
@@ -240,9 +241,9 @@ def test_tc_coverage():
 
 
 def test_position_invariance_case_lands_on_full_and_tail_tiles():
-    for engine in ('tc', 'ffma'):
-        b16 = oc.build(oc.with_batch(dict(oc.INVARIANCE, engine=engine), 16))
-        b3 = oc.build(oc.with_batch(dict(oc.INVARIANCE, engine=engine), 3))
+    for variant, engine in ((v, e) for v in oc.INVARIANCE_VARIANTS for e in ('tc', 'ffma')):
+        b16 = oc.build(oc.invariance(variant, engine, 16))
+        b3 = oc.build(oc.invariance(variant, engine, 3))
         o16, o3 = b16.pb.ops[b16.main], b3.pb.ops[b3.main]
         assert _kernel(b16, b16.main) == _kernel(b3, b3.main) != 'linear_small_m'
         if engine == 'tc':
@@ -258,8 +259,8 @@ def test_every_kernel_is_reached():
     for case in ALL.values():
         b = oc.build(_small(case))
         reached |= {_kernel(b, i) for i in _main_ops(b)}
-    want = {'conv_tc<tf32>', 'conv_tc<f16>', 'conv_ffma<32>', 'conv_ffma<64>', 'conv_ffma<128>', 'linear_small_m',
-            'conv_c1_wide', 'conv_c1', 'pool2d', 'ew', 'pad_copy', 'colstats', 'colstats_smem', 'asp', 'asp_smem'}
+    want = {'conv_tc<tf32>', 'conv_tc<tf32,add>', 'conv_tc<tf32,pre>', 'conv_tc<f16>', 'conv_ffma<32>', 'conv_ffma<64>',
+            'conv_ffma<128>', 'linear_small_m', 'conv_c1_wide', 'conv_c1', 'pool2d', 'ew', 'pad_copy', 'colstats', 'colstats_smem', 'asp', 'asp_smem'}
     assert want <= reached, want - reached
 
 
