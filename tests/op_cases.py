@@ -7,10 +7,10 @@ accumulate-into view, the columns around an output window) and, for the amax cas
 ``run_gpu`` runs the program through Program.run_profiled; ``Sim(pb, blob, X).run()`` (tests/plan_sim.py) is the
 fp64 reference.
 
-Every case names the kernel it is meant to reach (``kernel``) and, for convs, the engine it requests (``engine``);
-the GPU tests assert the engine from run_profiled, the CPU tests re-derive the kernel from the lowered op with the
-launchers' own predicates (``kernel_of``, ``tc_schedule``), so a table entry cannot drift into covering something else.
-Never imported by the product."""
+Every case names the kernel it is meant to reach (``kernel``) and, for convs, the engine it requests (``engine``;
+'auto' expects the engine ``engine_of`` resolves); the GPU tests assert the engine from run_profiled, the CPU tests
+re-derive the kernel from the lowered op with the launchers' own predicates (``kernel_of``, ``tc_schedule``), so a
+table entry cannot drift into covering something else.  Never imported by the product."""
 import os
 
 import numpy as np
@@ -19,7 +19,7 @@ from mvector import _lib as L
 from mvector.engine import PlanBuilder, View, WeightArena, tc_tile_n
 
 SMS = 132                                   # H100 SXM: the persistent tensor-core grid is min(SMs, tiles)
-ENGINES = {'ffma': L.ENGINE_FFMA, 'tc': L.ENGINE_TC, 'tc16': L.ENGINE_TC16}
+ENGINES = {'auto': L.ENGINE_AUTO, 'ffma': L.ENGINE_FFMA, 'tc': L.ENGINE_TC, 'tc16': L.ENGINE_TC16}
 ERES_POLICY = (512, 256)                    # models/eres2net.py: chunk K > 512 by 256
 DEFAULT_POLICY = (1536, 512)                # models/base.py
 
@@ -115,9 +115,10 @@ def _conv(pb, arena, inp, c, rng, expect, src=None, dst=None):
     elif c1:
         inp.take(rows_in, 1, fill=xfill)                       # the one-channel map is the flat start of the input
         src = View(L.BUF_INPUT, 1, 0, 1)
-    elif engine == 'tc16':
+    elif engine == 'tc16' and not c.get('raw_input'):
         # the fp16 split scales by the source tensor's tracked maximum: the source is a workspace tensor written by
-        # program ops; with a concat, both halves are windows of ONE allocation (two writers, one amax slot)
+        # program ops; with a concat, both halves are windows of ONE allocation (two writers, one amax slot).
+        # ``raw_input``: read the program input itself, which has no amax slot
         a = pb.alloc(rows_in, in_coff + Cin + Cin2)
         src = a.cols(in_coff, Cin)
         _copy(pb, inp.take(rows_in, Cin, fill=xfill), src, rows_in)
@@ -239,10 +240,11 @@ def _ew(pb, inp, c, dst=None):
 def _pool(pb, inp, c):
     """COLSTATS / ASP_POOL over B utterances x R rows of C columns."""
     B, R, C = c['B'], c['R'], c['C']
-    x = inp.take(B * R, C, fill=c.get('fill', ('normal', 2.0, 0.0)), skew=c.get('in_coff', 0))
+    skew = c.get('in_coff', 0)
+    x = inp.take(B * R, C, fill=c.get('fill', ('normal', 2.0, 0.0)), skew=skew)
     main = len(pb.ops)
     if c['op'] == 'asp':
-        logits = inp.take(B * R, C, fill=('normal', 2.0, c.get('logit_shift', 0.0)))
+        logits = inp.take(B * R, C, fill=('normal', 2.0, c.get('logit_shift', 0.0)), skew=skew)
         n_rows, n_cols = B, C if c.get('mean_only') else 2 * C
         pb.asp_pool(x, logits, pb.output_view(n_cols, n_rows), R, eps=1e-12, mean_only=c.get('mean_only', False))
     else:
@@ -304,6 +306,9 @@ def build(case):
     width = max(4, (_build(case, 1 << 16)[2].used + 3) // 4 * 4)
     pb, arena, inp, main, expect, consumer, out_rows, out_cols = _build(case, width)
     X = inp.data(np.random.default_rng(case['seed'] + 7919), case.get('scale', 1.0))
+    for i, e in expect.items():
+        if e == L.ENGINE_AUTO and pb.ops[i].kind == L.OP_CONV:
+            expect[i] = engine_of(pb.finalize().ops[i])
     b = Built(case, pb, arena, X, out_rows, out_cols, main, expect, consumer)
     for d in inp.derived:
         X[:d['rows'], d['col']:d['col'] + d['C']] = _gathered(X, b.blob, d)
@@ -529,13 +534,14 @@ def ew_grid_strides(o):
 # ---------------------------------------------------------------------------------------------------------------
 # case tables
 # ---------------------------------------------------------------------------------------------------------------
-def _tc(name, engines, **c):
-    """A tensor-core conv case, once per engine ('tc' = split TF32, 'tc16' = fp16 split, 'ffma' = exact reference)."""
+def _tc(name, engines, table=None, **c):
+    """A tensor-core conv case, once per engine ('tc' = split TF32, 'tc16' = fp16 split, 'ffma' = exact reference),
+    into ``table`` (TC_CASES by default)."""
     for e in engines:
         kern = {'tc': 'conv_tc<tf32%s>' % _tc_suffix(c.get('pre'), c.get('src2_mode') == L.SRC2_ADD),
                 'tc16': 'conv_tc<f16>',
                 'ffma': 'conv_ffma<%d>' % (128 if c['N'] > 64 else 64 if c['N'] > 32 else 32)}[e]
-        TC_CASES[f'{name}-{e}'] = dict(c, op='conv', engine=e, kernel=kern)
+        (TC_CASES if table is None else table)[f'{name}-{e}'] = dict(c, op='conv', engine=e, kernel=kern)
 
 
 TC_CASES = {}
@@ -659,6 +665,67 @@ INVARIANCE_VARIANTS = {'': {}, 'add': ADD, 'pre': PRE}
 def invariance(variant, engine, B):
     return dict(INVARIANCE, **INVARIANCE_VARIANTS[variant], engine=engine, B=B)
 
+
+# ---- the backbones' conv geometries on both engines, and on the fp16 split where N >= 128 and nothing but a plain
+# source feeds it: pointwise GEMMs, Res2 k3 convs with dilation, reflect padding and an added or accumulated second
+# source, stems, valid TDNN convs, 2-D 3x3 convs with stride / residual / concat, CAM++'s BN-ReLU prologue (uniform
+# scales) and per-segment gate, K chunked by the default policy, N and K tails ----
+ENGINE_CASES = {}
+_TC16_GEOMETRIES = {'gemm_512', 'gemm_n1536_k128', 'gemm_k1536_n128_ubias_tanh', 'stem_k5_reflect', 'tdnn_valid_k3_d3',
+                    'k5_stride2_zero', 'n_tail_192', 'long_k_chunked_9216', 'long_k_chunked_4096_n128'}
+for _name, _c in dict(
+        gemm_512=dict(seed=1, B=8, Tin=298, Cin=512, N=512, bias=True, act=L.ACT_RELU, post=True),
+        gemm_n1536_k128=dict(seed=2, B=5, Tin=298, Cin=128, N=1536, bias=True),
+        gemm_k1536_n128_ubias_tanh=dict(seed=3, B=6, Tin=211, Cin=1536, N=128, ubias=True, act=L.ACT_RELU, post=True,
+                                        act2=L.ACT_TANH),
+        res2_k3_dil2_reflect_add=dict(seed=4, B=9, Tin=298, Cin=64, N=64, KT=3, dT=2, padT=2, pad_mode=L.PAD_REFLECT,
+                                      bias=True, act=L.ACT_RELU, post=True, src2_mode=L.SRC2_ADD),
+        stem_k5_reflect=dict(seed=5, B=7, Tin=298, Cin=80, N=512, KT=5, padT=2, pad_mode=L.PAD_REFLECT, bias=True,
+                             act=L.ACT_RELU, post=True),
+        tdnn_valid_k3_d3=dict(seed=6, B=4, Tin=300, Tout=294, Cin=512, N=512, KT=3, dT=3, bias=True, act=L.ACT_RELU,
+                              post=True),
+        conv2d_3x3_s2=dict(seed=7, B=3, Tin=61, Fin=40, Tout=31, Fout=20, Cin=32, N=48, KT=3, KF=3, sT=2, sF=2, padT=1,
+                           padF=1, bias=True, act=L.ACT_HARDTANH20),
+        conv2d_3x3_res_relu=dict(seed=8, B=2, Tin=50, Fin=20, Cin=32, N=32, KT=3, KF=3, padT=1, padF=1, bias=True,
+                                 res=True, act2=L.ACT_RELU),
+        concat_1x1_silu=dict(seed=9, B=2, Tin=40, Fin=30, Cin=16, Cin2=16, N=16, bias=True, act=L.ACT_SILU,
+                             src2_mode=L.SRC2_CONCAT),
+        cam_pre_bn_relu=dict(seed=10, B=9, Tin=149, Cin=160, N=128, pre=True, bias=True, act=L.ACT_RELU),
+        cam_local_gate_seg=dict(seed=11, B=6, Tin=249, Cin=128, N=32, KT=3, dT=2, padT=2, gate=True, seg_len=100,
+                                n_seg=3),
+        k5_stride2_zero=dict(seed=12, B=8, Tin=298, Tout=149, Cin=320, N=128, KT=5, sT=2, padT=2, bias=True,
+                             act=L.ACT_RELU),
+        n_tail_192=dict(seed=13, B=3, Tin=400, Cin=96, N=192, bias=True),
+        long_k_chunked_9216=dict(seed=15, B=6, Tin=40, Fin=20, Tout=20, Fout=10, Cin=1024, N=256, KT=3, KF=3, sT=2,
+                                 sF=2, padT=1, padF=1),
+        long_k_chunked_4096_n128=dict(seed=16, B=7, Tin=151, Cin=4096, N=128, ubias=True, act=L.ACT_RELU, post=True,
+                                      act2=L.ACT_TANH),
+        res2_k3_dil3_reflect_sum=dict(seed=17, B=9, Tin=298, Cin=64, N=64, KT=3, dT=3, padT=3, pad_mode=L.PAD_REFLECT,
+                                      bias=True, act=L.ACT_RELU, post=True, sum=True),
+        conv2d_3x3_sum_hardtanh=dict(seed=18, B=2, Tin=50, Fin=20, Cin=16, N=16, KT=3, KF=3, padT=1, padF=1, bias=True,
+                                     act=L.ACT_HARDTANH20, sum=True),
+        k_tail_72=dict(seed=14, B=11, Tin=100, Cin=24, N=24, KT=3, padT=1, bias=True, act=L.ACT_HARDTANH20),
+).items():
+    _tc(_name, ('ffma', 'tc', 'tc16') if _name in _TC16_GEOMETRIES else ('ffma', 'tc'), table=ENGINE_CASES, **_c)
+
+# ---- engine routing: what AUTO resolves to where a tensor-core engine cannot take the op, and the explicit requests
+# vp_program_create refuses (VP_ERR_UNSUPPORTED; engine_of raises ValueError) rather than run differently ----
+REFUSED_CASES = {}
+# a BN-ReLU prologue combined with a second source: the tensor-core gather reads one source, so AUTO runs FFMA
+for _name, _c in dict(
+        pre_concat_1x1=dict(seed=21, B=9, Tin=149, Cin=96, Cin2=64, N=128, pre=True, bias=True, act=L.ACT_RELU,
+                            src2_mode=L.SRC2_CONCAT),
+        pre_add_k3=dict(seed=22, B=9, Tin=149, Cin=64, N=64, KT=3, padT=1, pre=True, bias=True, act=L.ACT_RELU,
+                        src2_mode=L.SRC2_ADD),
+).items():
+    _tc(_name, ('ffma',), table=ENGINE_CASES, **_c)
+    ENGINE_CASES[f'{_name}-auto'] = dict(ENGINE_CASES[f'{_name}-ffma'], engine='auto')
+    REFUSED_CASES[f'{_name}-tc'] = dict(_c, op='conv', engine='tc')
+# a conv reading the program input itself has no amax slot: AUTO runs split TF32
+_RAW = dict(op='conv', seed=23, B=8, Tin=200, Cin=256, N=256, raw_input=True)
+ENGINE_CASES['raw_input-auto'] = dict(_RAW, engine='auto', kernel='conv_tc<tf32>')
+REFUSED_CASES['raw_input-tc16'] = dict(_RAW, engine='tc16')
+
 FFMA_CASES = {}
 # linear_small_m_kernel: M <= 1024 pointwise linears (SE MLPs, ASP per-utterance bias, final FC)
 for _name, _c in dict(
@@ -748,6 +815,25 @@ GLUE_CASES = dict(
     seg_context_last_one_row_71=dict(op='colstats', kernel='colstats', stats='SEG_CONTEXT', B=2, R=701, C=36,
                                      seg_len=10),
 )
+# pooling on both sides of each shared-memory limit, C = 72.  ASP / mean-only SAP: both [T, 32] strips are staged up to
+# T = 800 (T * 256 B <= 200 KB)
+for _T in (400, 401, 800, 801):
+    _k = 'asp_smem' if _T <= 800 else 'asp'
+    GLUE_CASES[f'asp_T{_T}'] = dict(op='asp', kernel=_k, B=3, R=_T, C=72)
+    GLUE_CASES[f'sap_mean_T{_T}'] = dict(op='asp', kernel=_k, B=3, R=_T, C=72, mean_only=True)
+# colstats: the [R, 32] strip is staged up to R = 800 rows (R * 128 B <= 100 KB)
+for _stats in ('MEAN', 'MEAN_STD_CLAMP', 'MEAN_STD_UNBIASED', 'MEAN_STD_TSTP', 'MEAN_VAR_UNBIASED'):
+    for _R in (800, 801):
+        GLUE_CASES[f'colstats_{_stats.lower()}_R{_R}'] = dict(op='colstats', kernel='colstats_smem' if _R <= 800
+                                                              else 'colstats', stats=_stats, B=3, R=_R, C=72)
+# segment context: the segment sums are parked in shared memory up to 64 segments, two sweeps above
+for _n in (64, 65):
+    GLUE_CASES[f'seg_context_{_n}'] = dict(op='colstats', kernel='colstats', stats='SEG_CONTEXT', B=3, R=10 * _n - 5,
+                                           C=72, seg_len=10)
+# views that start one column into their matrix: no 16-byte staging, the global-memory kernels run
+GLUE_CASES['asp_unaligned_coff'] = dict(op='asp', kernel='asp', B=3, R=298, C=72, in_coff=1)
+GLUE_CASES['colstats_unaligned_coff'] = dict(op='colstats', kernel='colstats', stats='MEAN_STD_CLAMP', B=3, R=298, C=72,
+                                             in_coff=1)
 for _i, _c in enumerate(GLUE_CASES.values()):
     _c['seed'] = 300 + _i
 
@@ -791,3 +877,9 @@ SHARED_SLOT_CASES = {
 
 # slot reset between graph replays: EW copy -> TC16 conv, run at 1e30, then at 1e-30 through the captured graph
 GRAPH_RESET = dict(op='ew', mode='COPY', B=4, T=300, C=64, out_C=64, seed=440, kernel='ew', consumer=_CONSUMER)
+
+# one 512 x 512 GEMM over 8 x 298 rows (EW copy -> TC16 conv) at input scales 1e-30 ... 1e30: the fp16 split neither
+# overflows (|x| > 65504) nor loses small tensors to fp16 subnormals, its error does not depend on the magnitude
+TC16_RANGE_CASES = {f'gemm_512-{_s:g}': dict(op='ew', mode='COPY', B=8, T=298, C=512, out_C=512, seed=450, scale=_s,
+                                             kernel='ew', consumer=dict(B=8, T=298, N=512))
+                    for _s in (1e-30, 1e-8, 1e-3, 1e4, 1e9, 1e30)}

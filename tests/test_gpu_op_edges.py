@@ -1,11 +1,13 @@
 """Op-level GPU tests at the shapes and edges where the backbone kernels go wrong: the persistent tensor-core schedule
 (several tiles per CTA, 133 tiles on 132 SMs), M / N / K tails, accumulation-chunk remainders, reflect padding at the
-smallest map, the fp16 split's epilogues, the FFMA family (small-M linear, tiled conv, both 2-D stem kernels), the glue
-kernels (pool2d, ew, pad copy, colstats, ASP) and the amax tracking that keeps the fp16 split range-safe.
+smallest map, the fp16 split's epilogues, the backbones' conv geometries on every engine and the engine AUTO picks, the
+FFMA family (small-M linear, tiled conv, both 2-D stem kernels), the glue kernels (pool2d, ew, pad copy, colstats, ASP,
+on both sides of their shared-memory limits) and the amax tracking that keeps the fp16 split range-safe.
 
 Each case is one op (plus the copies that feed it) from tests/op_cases.py, compared with the fp64 interpreter
 (tests/plan_sim.py).  Gates: FFMA kernels 2e-5 relative to max(1, max|ref|); split TF32 / fp16 split 1e-4; max pooling
-and copies bit-exact.  Every conv asserts the engine it ran on, so a case cannot pass through a silent fallback.
+and copies bit-exact.  Every conv asserts the engine it ran on, so a case cannot pass through a silent fallback, and an
+engine request the op cannot take must be refused when the program is created.
 
 The errors quoted in the docstrings were measured on an H100 80GB HBM3 at 700 W; the whole module runs in about 50 s
 there."""
@@ -14,6 +16,7 @@ import pytest
 import torch
 
 import op_cases as oc
+from mvector import _lib as L
 
 pytestmark = pytest.mark.gpu
 
@@ -40,6 +43,29 @@ def test_conv_schedule_and_tails(name):
     err = _rel(got, ref)
     print(f'{name}: max-rel err {err:.2e}')
     assert err <= (2e-5 if case['engine'] == 'ffma' else 1e-4), err
+
+
+@pytest.mark.parametrize('name', list(oc.ENGINE_CASES))
+def test_conv_engines_on_backbone_geometries(name):
+    """The backbones' conv geometries on exact fp32 FFMA, split TF32 and (N >= 128) the fp16 split, and the engine AUTO
+    resolves to where a tensor-core engine cannot take the op (FFMA for a prologue with a second source, split TF32 on
+    the raw program input), gated by the engine that ran.  Measured max-rel error: FFMA <= 7.5e-6; split TF32 <= 3.7e-6
+    at K <= 512 and up to 4.1e-5 at K = 1536, the longest unchunked accumulation -- the tensor core's fp32 accumulator
+    truncates on every accumulate, a bias that does not average out, still 10-100x below single-pass TF32's ~1e-3;
+    fp16 split <= 2.2e-5 (K = 1536)."""
+    b, got, ref = _run(oc.ENGINE_CASES[name])
+    err = _rel(got, ref)
+    print(f'{name}: max-rel err {err:.2e}')
+    assert err <= (2e-5 if b.expect[b.main] == L.ENGINE_FFMA else 1e-4), err
+
+
+def test_unsupported_engine_requests_are_refused():
+    """An explicit tensor-core request the op cannot take (a prologue with a second source on split TF32, the fp16 split
+    on an untracked source) fails when the program is created: never a silently different result."""
+    for name, case in oc.REFUSED_CASES.items():
+        with pytest.raises(L.VpError):
+            oc.run_gpu(oc.build(case))
+            pytest.fail(f'{name}: the program was created and ran')
 
 
 @pytest.mark.parametrize('engine', ['tc', 'ffma', 'add-tc', 'add-ffma', 'pre-tc', 'pre-ffma'])
@@ -103,15 +129,19 @@ def test_glue_kernels(name):
         assert spread.max() <= 5e-2, spread.max()
 
 
-@pytest.mark.parametrize('name', list(oc.AMAX_CASES))
+SCALED = {**oc.AMAX_CASES, **oc.TC16_RANGE_CASES}
+
+
+@pytest.mark.parametrize('name', list(SCALED))
 def test_amax_writer_feeds_tc16(name):
     """Every kernel that writes a TC16 source reports max|y| into the source's amax slot: the consumer (1x1 TC16 conv)
-    must stay finite and fp32-grade at input scales 1e-30 ... 1e30 (inputs and writer biases both scaled).  A writer
-    that reports too small a maximum gives the consumer too large a scale, and its fp16 hi terms overflow at any
-    magnitude; a writer that reports nothing leaves the slot at 0, which means scale 1: overflow at the large scales,
-    flush to zero at the small ones.  (Too large a maximum -- an over-reporting writer, a stale slot -- flushes small
-    tensors to zero; see the graph-replay test.)  Measured max-rel error <= 1.7e-6."""
-    case = oc.AMAX_CASES[name]
+    must stay finite and fp32-grade at input scales 1e-30 ... 1e30 (inputs and writer biases both scaled), and so must
+    a 512 x 512 GEMM over 8 x 298 rows (the gemm_512 cases).  A writer that reports too small a maximum gives the
+    consumer too large a scale, and its fp16 hi terms overflow at any magnitude; a writer that reports nothing leaves
+    the slot at 0, which means scale 1: overflow at the large scales, flush to zero at the small ones.  (Too large a
+    maximum -- an over-reporting writer, a stale slot -- flushes small tensors to zero; see the graph-replay test.)
+    Measured max-rel error <= 1.7e-6 (2.3e-6 on the 512 x 512 GEMM)."""
+    case = SCALED[name]
     b, got, ref = _run(case)
     assert b.pb.ops[b.consumer].amax_in > 0
     assert np.isfinite(got).all()
@@ -133,7 +163,6 @@ def test_amax_slot_shared_by_column_windows(order):
 def test_amax_slots_reset_between_graph_replays():
     """vp_embed replays a CUDA graph from its second call on; the graph's memset node must zero the amax slots, or a
     1e-30 input run after a 1e30 one is scaled by the stale maximum and flushes to zero in fp16."""
-    from mvector import _lib as L
     from mvector.engine import Engine, Program
     big = oc.build(dict(oc.GRAPH_RESET, scale=1e30))
     small = oc.build(dict(oc.GRAPH_RESET, scale=1e-30))

@@ -4,8 +4,10 @@
   torch evaluation of the same program -- F.conv2d over an explicit reflect / zero F.pad, F.max_pool2d /
   F.avg_pool2d(count_include_pad=True), softmax-weighted statistics, torch.var, the AFF formula;
 * coverage intent: every case reaches the kernel it names (the launchers' predicates, mirrored with their source lines
-  in op_cases.kernel_of / tc_schedule), the tile / chunk schedules the tables claim, and the amax slots the fp16 split
-  relies on."""
+  in op_cases.kernel_of / tc_schedule) on the engine it requests, the tile / chunk schedules the tables claim, and the
+  amax slots the fp16 split relies on;
+* the engine requests the library refuses (op_cases.REFUSED_CASES) are refused by the engine mirror
+  (op_cases.engine_of)."""
 import numpy as np
 import pytest
 import torch
@@ -14,9 +16,12 @@ import torch.nn.functional as F
 import op_cases as oc
 from mvector import _lib as L
 
-ALL = {**{f'tc/{k}': v for k, v in oc.TC_CASES.items()}, **{f'ffma/{k}': v for k, v in oc.FFMA_CASES.items()},
+ALL = {**{f'tc/{k}': v for k, v in oc.TC_CASES.items()}, **{f'engine/{k}': v for k, v in oc.ENGINE_CASES.items()},
+       **{f'ffma/{k}': v for k, v in oc.FFMA_CASES.items()},
        **{f'glue/{k}': v for k, v in oc.GLUE_CASES.items()}, **{f'amax/{k}': v for k, v in oc.AMAX_CASES.items()},
-       **{f'shared/{k}': v for k, v in oc.SHARED_SLOT_CASES.items()}, 'graph/reset': oc.GRAPH_RESET}
+       **{f'shared/{k}': v for k, v in oc.SHARED_SLOT_CASES.items()}, 'graph/reset': oc.GRAPH_RESET,
+       **{f'range/{k}': v for k, v in oc.TC16_RANGE_CASES.items()}}
+SCALED = {**oc.AMAX_CASES, **oc.TC16_RANGE_CASES}
 
 
 # ---------------------------------------------------------------------------------------------------------------
@@ -186,7 +191,15 @@ def _kernel(b, i):
 @pytest.mark.parametrize('name', [n for n in ALL if ALL[n].get('kernel')])
 def test_case_reaches_its_kernel(name):
     b = oc.build(ALL[name])
+    assert oc.engine_of(b.pb.finalize().ops[b.main]) == b.expect.get(b.main, 0)     # the request is not refused
     assert _kernel(b, b.main) == ALL[name]['kernel']
+
+
+@pytest.mark.parametrize('name', list(oc.REFUSED_CASES))
+def test_engine_mirror_refuses_unsupported_request(name):
+    b = oc.build(oc.REFUSED_CASES[name])
+    with pytest.raises(ValueError):
+        oc.engine_of(b.pb.finalize().ops[b.main])
 
 
 def _schedules():
@@ -307,11 +320,11 @@ def test_amax_slots_link_writer_and_consumer(name):
         assert b.pb.ops[i].amax_out == consumer.amax_in, (name, i)
 
 
-@pytest.mark.parametrize('name', list(oc.AMAX_CASES))
+@pytest.mark.parametrize('name', list(SCALED))
 def test_amax_consumer_sees_the_scale(name):
     """At every scale of the sweep, the tensor the TC16 consumer reads -- and hence its output -- is O(scale): nothing
     unscaled (a bias, a residual) pulls the small-scale cases back to unit magnitude."""
-    case = oc.AMAX_CASES[name]
+    case = SCALED[name]
     peak = np.abs(oc.sim(oc.build(case))).max() / case['scale']
     assert 1e-2 <= peak <= 1e3, peak
 
