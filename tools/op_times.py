@@ -1,4 +1,5 @@
-"""Per-op device times of the ECAPA B=256 program (dev tool)."""
+"""Per-op device times of the ECAPA B=256 program (dev tool): the mean time of each tensor-core conv class
+(engine, M x N x K) over three profiled runs."""
 import json, sys, collections
 sys.path.insert(0, '.')
 import torch
@@ -28,4 +29,5 @@ for o in acc:
     key = (o['kind'], o['engine'], o['M'], o['N'], o['K'])
     a = agg.setdefault(key, [0, 0.0]); a[0] += 1; a[1] += o['ms'] / 3
 tot = sum(v[1] for v in agg.values())
-print('total %.3f ms' % tot, ' | '.join(f"{k[3]}x{k[4]}:{v[1]/v[0]:.3f}" for k, v in agg.items() if k[0] == 1 and k[1] == 2))
+print('total %.3f ms' % tot, ' | '.join(f"{'tf32' if k[1] == 2 else 'fp16'} {k[2]}x{k[3]}x{k[4]}:{v[1]/v[0]:.3f}"
+                                        for k, v in agg.items() if k[0] == 1 and k[1] in (2, 3)))

@@ -21,6 +21,8 @@
 //                           as the stage is free, lands B_hi|B_lo
 // Pipeline: S shared-memory stages (full/empty mbarriers); a stage is released as soon as the wgmma group that read
 // it has retired, while the next K block's group is already in flight.
+#include <cuda.h>
+#include <cudaTypedefs.h>
 #include <cuda_fp16.h>
 
 #include <cstdlib>
@@ -124,6 +126,129 @@ __device__ __forceinline__ void mma_tile(float* d, uint32_t a, uint32_t b, uint3
 __device__ __noinline__ float2 act2_slow(float2 v, int act) {
   v.x = apply_act(v.x, act); v.y = apply_act(v.y, act);
   return v;
+}
+
+// Per-launch epilogue flags.  ReLU and the ERes2Net family's ReLU(20) = Hardtanh(0, 20) (eres2net.py:12-17) are both
+// "clamp to [0, hi]" with hi = +inf / 20: min(max(x, 0), hi), the same expression and order as apply_act.
+struct Epi {
+  bool simple, relu, relu2, need_urow;
+  float hi1, hi2;
+  float descale;         // fp16 split: 2^-k of the weight image x 2^-s of the activation scale; 1 on the tf32 path
+};
+__device__ __forceinline__ Epi make_epi(const ConvParams& p, float descale) {
+  auto clamps = [](int act) { return act == VP_ACT_RELU || act == VP_ACT_HARDTANH20; };
+  Epi e;
+  e.simple = !p.ubias && !p.gate && !p.sum && (p.act == VP_ACT_NONE || clamps(p.act)) &&
+             (p.act2 == VP_ACT_NONE || clamps(p.act2));
+  e.relu = clamps(p.act);
+  e.relu2 = clamps(p.act2);
+  e.hi1 = p.act == VP_ACT_HARDTANH20 ? 20.f : INFINITY;
+  e.hi2 = p.act2 == VP_ACT_HARDTANH20 ? 20.f : INFINITY;
+  e.need_urow = (p.gate != nullptr) || (p.ubias != nullptr);
+  e.descale = descale;
+  return e;
+}
+
+// Residual tiles are pure streaming: pull tile gg's residual rows (this consumer warp's 16) into the L2 while the
+// current tile's MMAs run, so that the epilogue's residual loads are L2 hits.
+template <int BN>
+__device__ __forceinline__ void prefetch_res(const ConvParams& p, int gg, int n_tiles, int warp, int lane) {
+  if (!p.res) return;
+  const int mr = (gg / n_tiles) * BM + 64 * (warp >> 2) + 16 * (warp & 3) + (lane & 15);
+  const float* base = p.res + p.res_coff + (gg % n_tiles) * BN;
+  if (mr < p.M)
+    for (int c = 32 * (lane >> 4); c < BN; c += 64)
+      asm volatile("prefetch.global.L2 [%0];" ::"l"(base + (size_t)mr * p.res_ld + c));
+}
+
+// Fused epilogue of one consumer thread's share of a BM x BN tile, straight from the wgmma accumulator fragments
+// (res[4j + 2h + c] = row ma + 8h, column n0 + 8j + 2 q4 + c): every float2 store of a quad of lanes covers one whole
+// 32-byte sector of an output row.  tmax collects max |y| of what is stored (amax_out slot).
+template <int BN>
+__device__ __forceinline__ void store_tile(const ConvParams& p, const Epi& e, const float (&res)[BN / 2], int m0, int n0,
+                                           int ma, int q4, float& tmax) {
+  const float descale = e.descale;
+  if (e.simple && m0 + BM <= p.M && n0 + BN <= p.N) {
+    // Fast path: the common epilogue shape -- bias, optional ReLU, optional BN affine, optional residual, nothing
+    // per utterance -- on a tile without row / column tails needs no predicates and three FP instructions per element.
+    float* o = p.dst + (size_t)ma * p.out_ld + p.out_coff + n0 + 2 * q4;
+    const float* rp = p.res ? p.res + (size_t)ma * p.res_ld + p.res_coff + n0 + 2 * q4 : nullptr;
+    const size_t o8 = (size_t)8 * p.out_ld, r8 = (size_t)8 * p.res_ld;
+#pragma unroll
+    for (int j = 0; j < BN / 8; ++j) {
+      const int n = n0 + 8 * j + 2 * q4;
+      float2 b2 = make_float2(0.f, 0.f), s2 = make_float2(1.f, 1.f), h2 = b2;
+      if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+      if (p.post_s) {
+        s2 = __ldg(reinterpret_cast<const float2*>(p.post_s + n));
+        h2 = __ldg(reinterpret_cast<const float2*>(p.post_h + n));
+      }
+      float2 rr[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
+      if (rp) {
+        rr[0] = __ldg(reinterpret_cast<const float2*>(rp + 8 * j));
+        rr[1] = __ldg(reinterpret_cast<const float2*>(rp + 8 * j + r8));
+      }
+#pragma unroll
+      for (int h = 0; h < 2; ++h) {
+        float2 x = make_float2(res[4 * j + 2 * h], res[4 * j + 2 * h + 1]);
+        x.x = fmaf(x.x, descale, b2.x); x.y = fmaf(x.y, descale, b2.y);      // descale == 1 on the tf32 path
+        if (e.relu) { x.x = fminf(fmaxf(x.x, 0.f), e.hi1); x.y = fminf(fmaxf(x.y, 0.f), e.hi1); }
+        if (p.post_s) { x.x = fmaf(x.x, s2.x, h2.x); x.y = fmaf(x.y, s2.y, h2.y); }
+        if (rp) { x.x += rr[h].x; x.y += rr[h].y; }
+        if (e.relu2) { x.x = fminf(fmaxf(x.x, 0.f), e.hi2); x.y = fminf(fmaxf(x.y, 0.f), e.hi2); }
+        *reinterpret_cast<float2*>(o + 8 * j + h * o8) = x;
+        tmax = fmaxf(tmax, fmaxf(fabsf(x.x), fabsf(x.y)));
+      }
+    }
+    return;
+  }
+  // General epilogue: row / column tails and the per-utterance / gated / accumulate-into layers.
+#pragma unroll
+  for (int j = 0; j < BN / 8; ++j) {
+    const int n = n0 + 8 * j + 2 * q4;
+    if (n >= p.N) continue;              // N % 4 == 0: n < N implies n + 1 < N
+    float2 b2 = make_float2(0.f, 0.f), s2 = make_float2(1.f, 1.f), h2 = b2;
+    if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n));
+    if (p.post_s) {
+      s2 = __ldg(reinterpret_cast<const float2*>(p.post_s + n));
+      h2 = __ldg(reinterpret_cast<const float2*>(p.post_h + n));
+    }
+#pragma unroll
+    for (int h = 0; h < 2; ++h) {
+      const int m = ma + 8 * h;
+      if (m >= p.M) continue;
+      float2 x = make_float2(res[4 * j + 2 * h], res[4 * j + 2 * h + 1]);
+      // acc * descale + bias in one rounding (descale == 1 on the tf32 path: exactly acc + bias) -- the same
+      // expression as the fast path, so a row's result does not depend on which path its tile took
+      x.x = fmaf(x.x, descale, b2.x); x.y = fmaf(x.y, descale, b2.y);
+      const int ur = e.need_urow ? urow_of(p, m) : 0;
+      if (p.ubias) {
+        const float2 u = __ldg(reinterpret_cast<const float2*>(p.ubias + (size_t)ur * p.N + n));
+        x.x += u.x; x.y += u.y;
+      }
+      if (p.act == VP_ACT_RELU) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); }
+      else if (p.act != VP_ACT_NONE) x = act2_slow(x, p.act);
+      if (p.post_s) { x.x = fmaf(x.x, s2.x, h2.x); x.y = fmaf(x.y, s2.y, h2.y); }
+      if (p.gate) {
+        const float2 gt = __ldg(reinterpret_cast<const float2*>(p.gate + (size_t)ur * p.N + n));
+        x.x *= gt.x; x.y *= gt.y;
+      }
+      if (p.res) {
+        const float2 r = __ldg(reinterpret_cast<const float2*>(p.res + (size_t)m * p.res_ld + p.res_coff + n));
+        x.x += r.x; x.y += r.y;
+      }
+      if (p.act2 == VP_ACT_RELU) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); }
+      else if (p.act2 != VP_ACT_NONE) x = act2_slow(x, p.act2);
+      *reinterpret_cast<float2*>(p.dst + (size_t)m * p.out_ld + p.out_coff + n) = x;
+      tmax = fmaxf(tmax, fmaxf(fabsf(x.x), fabsf(x.y)));
+      if (p.sum) {                         // accumulate-into view (Res2 chains): sum[m, n] += y[m, n]
+        float2* sq = reinterpret_cast<float2*>(p.sum + (size_t)m * p.sum_ld + p.sum_coff + n);
+        float2 sv = *sq;
+        sv.x += x.x; sv.y += x.y;
+        *sq = sv;
+      }
+    }
+  }
 }
 
 template <int MODE> struct Slot;
@@ -369,27 +494,11 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
     float descale = 1.f;                                      // fp16 split: 2^-k of the weight image x 2^-s of the activation scale
     if constexpr (F16) descale = a.descale * exp2i(-f16_scale_exp(__ldg(p.amax_in)));
     float tmax = 0.f;                                         // running max |y| of everything this thread stores (amax_out slot)
-    auto clamps = [](int act) { return act == VP_ACT_RELU || act == VP_ACT_HARDTANH20; };
-    // ReLU and the ERes2Net family's ReLU(20) = Hardtanh(0, 20) (eres2net.py:12-17) are both "clamp to [0, hi]" with
-    // hi = +inf / 20: min(max(x, 0), hi), the same expression and order as apply_act.
-    const bool simple = !p.ubias && !p.gate && !p.sum && (p.act == VP_ACT_NONE || clamps(p.act)) &&
-                        (p.act2 == VP_ACT_NONE || clamps(p.act2));
-    const bool relu = clamps(p.act), relu2 = clamps(p.act2);
-    const float hi1 = p.act == VP_ACT_HARDTANH20 ? 20.f : INFINITY, hi2 = p.act2 == VP_ACT_HARDTANH20 ? 20.f : INFINITY;
-    const bool need_urow = (p.gate != nullptr) || (p.ubias != nullptr);
+    const Epi epi = make_epi(p, descale);
     for (int g = blockIdx.x; g < total_groups; g += gridDim.x) {
       const int m0 = (g / a.n_tiles) * BM;
       const int n0 = (g % a.n_tiles) * BN;
-      if (p.res && g + (int)gridDim.x < total_groups) {
-        // residual tiles are pure streaming: pull the NEXT tile's residual rows (this warp's 16) into the L2 while this
-        // tile's MMAs run, so that the epilogue's residual loads are L2 hits
-        const int gg = g + gridDim.x;
-        const int mr = (gg / a.n_tiles) * BM + 64 * wg + 16 * (warp & 3) + (lane & 15);
-        const float* base = p.res + p.res_coff + (gg % a.n_tiles) * BN;
-        if (mr < p.M)
-          for (int c = 32 * (lane >> 4); c < BN; c += 64)
-            asm volatile("prefetch.global.L2 [%0];" ::"l"(base + (size_t)mr * p.res_ld + c));
-      }
+      if (g + (int)gridDim.x < total_groups) prefetch_res<BN>(p, g + gridDim.x, a.n_tiles, warp, lane);
       // Long-K layers are accumulated in chunks of `kc` K blocks, each into a fresh accumulator that is then folded
       // into a running fp32 sum with correctly rounded adds.  (The tensor core truncates on every accumulate; the bias
       // grows linearly with the number of accumulates.)
@@ -434,88 +543,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
           }
         }
       }
-      const int ma = m0 + rbase;
-      if (simple && m0 + BM <= p.M && n0 + BN <= p.N) {
-        // Fast path: the common epilogue shape -- bias, optional ReLU, optional BN affine, optional residual, nothing
-        // per utterance -- on a tile without row / column tails needs no predicates and three FP instructions per element.
-        float* o = p.dst + (size_t)ma * p.out_ld + p.out_coff + n0 + 2 * q4;
-        const float* rp = p.res ? p.res + (size_t)ma * p.res_ld + p.res_coff + n0 + 2 * q4 : nullptr;
-        const size_t o8 = (size_t)8 * p.out_ld, r8 = (size_t)8 * p.res_ld;
-#pragma unroll
-        for (int j = 0; j < BN / 8; ++j) {
-          const int n = n0 + 8 * j + 2 * q4;
-          float2 b2 = make_float2(0.f, 0.f), s2 = make_float2(1.f, 1.f), h2 = b2;
-          if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-          if (p.post_s) {
-            s2 = __ldg(reinterpret_cast<const float2*>(p.post_s + n));
-            h2 = __ldg(reinterpret_cast<const float2*>(p.post_h + n));
-          }
-          float2 rr[2] = {make_float2(0.f, 0.f), make_float2(0.f, 0.f)};
-          if (rp) {
-            rr[0] = __ldg(reinterpret_cast<const float2*>(rp + 8 * j));
-            rr[1] = __ldg(reinterpret_cast<const float2*>(rp + 8 * j + r8));
-          }
-#pragma unroll
-          for (int h = 0; h < 2; ++h) {
-            float2 x = make_float2(res[4 * j + 2 * h], res[4 * j + 2 * h + 1]);
-            x.x = fmaf(x.x, descale, b2.x); x.y = fmaf(x.y, descale, b2.y);      // descale == 1 on the tf32 path
-            if (relu) { x.x = fminf(fmaxf(x.x, 0.f), hi1); x.y = fminf(fmaxf(x.y, 0.f), hi1); }
-            if (p.post_s) { x.x = fmaf(x.x, s2.x, h2.x); x.y = fmaf(x.y, s2.y, h2.y); }
-            if (rp) { x.x += rr[h].x; x.y += rr[h].y; }
-            if (relu2) { x.x = fminf(fmaxf(x.x, 0.f), hi2); x.y = fminf(fmaxf(x.y, 0.f), hi2); }
-            *reinterpret_cast<float2*>(o + 8 * j + h * o8) = x;
-            tmax = fmaxf(tmax, fmaxf(fabsf(x.x), fabsf(x.y)));
-          }
-        }
-        continue;
-      }
-      // General epilogue: row / column tails and the per-utterance / gated / accumulate-into layers.
-#pragma unroll
-      for (int j = 0; j < BN / 8; ++j) {
-        const int n = n0 + 8 * j + 2 * q4;
-        if (n >= p.N) continue;              // N % 4 == 0: n < N implies n + 1 < N
-        float2 b2 = make_float2(0.f, 0.f), s2 = make_float2(1.f, 1.f), h2 = b2;
-        if (p.bias) b2 = __ldg(reinterpret_cast<const float2*>(p.bias + n));
-        if (p.post_s) {
-          s2 = __ldg(reinterpret_cast<const float2*>(p.post_s + n));
-          h2 = __ldg(reinterpret_cast<const float2*>(p.post_h + n));
-        }
-#pragma unroll
-        for (int h = 0; h < 2; ++h) {
-          const int m = ma + 8 * h;
-          if (m >= p.M) continue;
-          float2 x = make_float2(res[4 * j + 2 * h], res[4 * j + 2 * h + 1]);
-          // acc * descale + bias in one rounding (descale == 1 on the tf32 path: exactly acc + bias) -- the same
-          // expression as the fast path, so a row's result does not depend on which path its tile took
-          x.x = fmaf(x.x, descale, b2.x); x.y = fmaf(x.y, descale, b2.y);
-          const int ur = need_urow ? urow_of(p, m) : 0;
-          if (p.ubias) {
-            const float2 u = __ldg(reinterpret_cast<const float2*>(p.ubias + (size_t)ur * p.N + n));
-            x.x += u.x; x.y += u.y;
-          }
-          if (p.act == VP_ACT_RELU) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); }
-          else if (p.act != VP_ACT_NONE) x = act2_slow(x, p.act);
-          if (p.post_s) { x.x = fmaf(x.x, s2.x, h2.x); x.y = fmaf(x.y, s2.y, h2.y); }
-          if (p.gate) {
-            const float2 gt = __ldg(reinterpret_cast<const float2*>(p.gate + (size_t)ur * p.N + n));
-            x.x *= gt.x; x.y *= gt.y;
-          }
-          if (p.res) {
-            const float2 r = __ldg(reinterpret_cast<const float2*>(p.res + (size_t)m * p.res_ld + p.res_coff + n));
-            x.x += r.x; x.y += r.y;
-          }
-          if (p.act2 == VP_ACT_RELU) { x.x = fmaxf(x.x, 0.f); x.y = fmaxf(x.y, 0.f); }
-          else if (p.act2 != VP_ACT_NONE) x = act2_slow(x, p.act2);
-          *reinterpret_cast<float2*>(p.dst + (size_t)m * p.out_ld + p.out_coff + n) = x;
-          tmax = fmaxf(tmax, fmaxf(fabsf(x.x), fabsf(x.y)));
-          if (p.sum) {                         // accumulate-into view (Res2 chains): sum[m, n] += y[m, n]
-            float2* sq = reinterpret_cast<float2*>(p.sum + (size_t)m * p.sum_ld + p.sum_coff + n);
-            float2 sv = *sq;
-            sv.x += x.x; sv.y += x.y;
-            *sq = sv;
-          }
-        }
-      }
+      store_tile<BN>(p, epi, res, m0, n0, m0 + rbase, q4, tmax);
     }
     if (p.amax_out) amax_commit(p.amax_out, tmax);     // one atomicMax per consumer warp per launch
   }
@@ -555,6 +583,174 @@ static cudaError_t launch_mode(const cudaLaunchConfig_t& cfg, const ConvParams& 
   }
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Wide FP16-split path for pointwise convs (launch_conv_tc16, tc16_wide_ok): 128 x 256 output tiles.
+//
+// The 128 x 128 kernel above pulls 64 KB from the L2 per 2.1 MFLOP stage (A as fp32 gathered by 256 producer threads,
+// B as the hi|lo fp16 image) and is L2-bandwidth bound.  A pointwise conv's A tile is a plain 2-D box of the channel-last
+// [M, K] view, so here one thread loads it with TMA (zero fill gives the M and K tails), the consumer warps split it into
+// fp16 hi / lo in registers (the same arithmetic as publish() above) and issue wgmma with A from registers, and the freed
+// registers hold a 256-wide accumulator: 96 KB of L2 traffic per 4.2 MFLOP stage.
+//   warps 0-7  consumers : two warpgroups of 64 rows, 232 registers each (setmaxnreg), 128 fp32 accumulators
+//   warps 8-11 producer  : one thread issues the stage's two A boxes and four B copies onto the stage's `full` mbarrier
+// B stage = n-tiles 2j and 2j + 1 of the 128-wide fp16 image at the same K block: hi | hi | lo | lo, so that B_hi and B_lo
+// each are 256 contiguous swizzled rows.  The three MMAs per K16 step run in the order of the 128-wide kernel
+// (A_lo B_hi, A_hi B_lo, A_hi B_hi) into one accumulator, so its first 128 columns equal that kernel's bit for bit.
+constexpr int WBN = 256;
+constexpr int W_A_BOX = BM * 128;                 // 16 KB: one TMA box of 128 rows x 32 fp32 (one SWIZZLE_128B row each)
+constexpr int W_A_STAGE = 2 * W_A_BOX;            // 64 K elements of fp32 A
+constexpr int W_B_HALF = WBN * 128;               // 32 KB: 256 rows x 64 fp16 (B_hi or B_lo)
+constexpr int W_STAGE = W_A_STAGE + 2 * W_B_HALF; // 96 KB
+constexpr int W_STAGES = 2;
+constexpr int W_THREADS = CONSUMER_THREADS + 128;
+constexpr int W_SMEM = W_STAGES * W_STAGE + 1024;
+
+struct WideArgs {
+  const uint8_t* w_tc16;  // the 128-wide fp16 image: [n_tile][k_block][hi 128 x 128 B | lo 128 x 128 B]
+  int m_tiles, n_tiles, k_blocks;  // n_tiles of 256 columns; k_blocks of 64
+  float descale;
+};
+
+__device__ __forceinline__ void tma_load_2d(uint32_t dst, const CUtensorMap* map, int c0, int c1, uint32_t bar) {
+  asm volatile(
+      "cp.async.bulk.tensor.2d.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1, {%2, %3}], [%4];" ::"r"(dst),
+      "l"(reinterpret_cast<uint64_t>(map)), "r"(c0), "r"(c1), "r"(bar)
+      : "memory");
+}
+
+// fp32 pair -> fp16 hi and lo terms of x * ascale, op for op as publish() above
+__device__ __forceinline__ void split_f16(float2 x, float ascale, uint32_t& hw, uint32_t& lw) {
+  const float x0 = x.x * ascale, x1 = x.y * ascale;
+  const __half2 h = __floats2half2_rn(x0, x1);
+  const float2 hf = __half22float2(h);
+  const __half2 l = __floats2half2_rn(x0 - hf.x, x1 - hf.y);
+  hw = *reinterpret_cast<const uint32_t*>(&h);
+  lw = *reinterpret_cast<const uint32_t*>(&l);
+}
+
+// One consumer warpgroup's K block (64 K = 4 x K16) of a stage: load its 64 rows of fp32 A from the swizzled stage,
+// split, and issue the 12 wgmmas as one group.  ah / al must stay untouched until that group has retired.
+__device__ __forceinline__ void wide_kblock(float (&acc)[WBN / 2], uint32_t (&ah)[4][4], uint32_t (&al)[4][4],
+                                            uint32_t a_rows, uint32_t b_hi, int q4, float ascale, bool first) {
+  const uint32_t sw = a_rows >> 7 & 7;   // the fragment's rows r and r + 8 share r & 7
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    const uint32_t half = a_rows + (kk >> 1) * W_A_BOX;
+    const uint32_t c = (kk & 1) * 4 + (q4 >> 1);         // 16-byte chunk of columns 16 (kk & 1) + 2 q4 (+1)
+    const uint32_t lo8 = (q4 & 1) * 8;
+    float2 x[4];
+    // (r, c), (r + 8, c), (r, c + 8 columns = 2 chunks), (r + 8, c + 2 chunks)
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x[0].x), "=f"(x[0].y) : "r"(half + ((c ^ sw) << 4) + lo8));
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x[1].x), "=f"(x[1].y) : "r"(half + 1024 + ((c ^ sw) << 4) + lo8));
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x[2].x), "=f"(x[2].y) : "r"(half + (((c + 2) ^ sw) << 4) + lo8));
+    asm volatile("ld.shared.v2.f32 {%0, %1}, [%2];" : "=f"(x[3].x), "=f"(x[3].y) : "r"(half + 1024 + (((c + 2) ^ sw) << 4) + lo8));
+#pragma unroll
+    for (int i = 0; i < 4; ++i) split_f16(x[i], ascale, ah[kk][i], al[kk][i]);
+  }
+  wgmma_fence();
+  const uint32_t b_lo = b_hi + W_B_HALF;
+#pragma unroll
+  for (int kk = 0; kk < 4; ++kk) {
+    wgmma_f16_rs_n256(acc, al[kk], smem_desc(b_hi + kk * 32), (first && kk == 0) ? 0u : 1u);
+    wgmma_f16_rs_n256(acc, ah[kk], smem_desc(b_lo + kk * 32), 1u);
+    wgmma_f16_rs_n256(acc, ah[kk], smem_desc(b_hi + kk * 32), 1u);
+  }
+  wgmma_commit();
+}
+
+__global__ void __launch_bounds__(W_THREADS, 1) conv_tc16_wide_kernel(const __grid_constant__ ConvParams p,
+                                                                      const __grid_constant__ WideArgs a,
+                                                                      const __grid_constant__ CUtensorMap amap) {
+  pdl_launch_dependents();
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t bars[2 * W_STAGES];     // full[S], empty[S]
+  const int warp = threadIdx.x >> 5;
+  const int lane = threadIdx.x & 31;
+  const uint32_t smem_base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[W_STAGES]);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < W_STAGES; ++s) {
+      mbar_init(full0 + 8 * s, 1);                        // the producer's expect_tx arrival; TMA completes the bytes
+      mbar_init(empty0 + 8 * s, CONSUMER_WARPS);          // one arrival per consumer warp once its wgmmas retired
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  __syncthreads();
+  pdl_wait();
+  const int total = a.m_tiles * a.n_tiles;
+
+  if (warp >= CONSUMER_WARPS) {
+    // =========================== producer ===========================
+    asm volatile("setmaxnreg.dec.sync.aligned.u32 24;" ::: "memory");
+    if (warp != CONSUMER_WARPS || lane != 0) return;
+    asm volatile("prefetch.tensormap [%0];" ::"l"(reinterpret_cast<uint64_t>(&amap)) : "memory");
+    constexpr uint32_t img_half = 128u * 128u;                 // hi (or lo) of one 128-wide image tile
+    int s = 0;
+    uint32_t ph = 0;
+    for (int g = blockIdx.x; g < total; g += gridDim.x) {
+      const int m0 = (g / a.n_tiles) * BM;
+      const int nt = g % a.n_tiles;
+      for (int kb = 0; kb < a.k_blocks; ++kb) {
+        mbar_wait(empty0 + 8 * s, ph ^ 1);
+        const uint32_t st = smem_base + s * W_STAGE, bar = full0 + 8 * s;
+        mbar_expect_tx(bar, W_STAGE);
+        tma_load_2d(st, &amap, kb * 64, m0, bar);
+        tma_load_2d(st + W_A_BOX, &amap, kb * 64 + 32, m0, bar);
+        const uint8_t* t0 = a.w_tc16 + ((size_t)(2 * nt) * a.k_blocks + kb) * (2u * img_half);
+        const uint8_t* t1 = t0 + (size_t)a.k_blocks * (2u * img_half);   // n-tile 2 nt + 1, same K block
+        const uint32_t b = st + W_A_STAGE;
+        bulk_copy_g2s(b, t0, img_half, bar);
+        bulk_copy_g2s(b + img_half, t1, img_half, bar);
+        bulk_copy_g2s(b + W_B_HALF, t0 + img_half, img_half, bar);
+        bulk_copy_g2s(b + W_B_HALF + img_half, t1 + img_half, img_half, bar);
+        if (++s == W_STAGES) { s = 0; ph ^= 1u; }
+      }
+    }
+    return;
+  }
+  // =========================== consumers: split + wgmma + epilogue ===========================
+  asm volatile("setmaxnreg.inc.sync.aligned.u32 240;" ::: "memory");
+  const int wg = warp >> 2;
+  const int q4 = lane & 3;
+  const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // fragment rows rbase and rbase + 8 of the tile
+  const int sexp = f16_scale_exp(__ldg(p.amax_in));
+  const float ascale = exp2i(sexp);
+  const Epi epi = make_epi(p, a.descale * exp2i(-sexp));
+  float acc[WBN / 2];
+#pragma unroll
+  for (int i = 0; i < WBN / 2; ++i) acc[i] = 0.f;
+  // two fragment sets, alternating by K block: a K block's set is rewritten only after wgmma_wait<1> in the next K block
+  // has retired the group that read it
+  uint32_t ah0[4][4], al0[4][4], ah1[4][4], al1[4][4];
+  float tmax = 0.f;
+  int s = 0;
+  uint32_t sph = 0;
+  for (int g = blockIdx.x; g < total; g += gridDim.x) {
+    const int m0 = (g / a.n_tiles) * BM;
+    const int n0 = (g % a.n_tiles) * WBN;
+    if (g + (int)gridDim.x < total) prefetch_res<WBN>(p, g + gridDim.x, a.n_tiles, warp, lane);
+    int prev = -1;
+    for (int kb = 0; kb < a.k_blocks; ++kb) {
+      mbar_wait(full0 + 8 * s, sph);
+      const uint32_t st = smem_base + s * W_STAGE;
+      const uint32_t a_rows = st + (uint32_t)rbase * 128u;
+      if (kb & 1) wide_kblock(acc, ah1, al1, a_rows, st + W_A_STAGE, q4, ascale, false);
+      else wide_kblock(acc, ah0, al0, a_rows, st + W_A_STAGE, q4, ascale, kb == 0);
+      if (prev >= 0) {                     // the previous K block's group has retired: release its stage
+        wgmma_wait<1>();
+        if (lane == 0) mbar_arrive(empty0 + 8 * prev);
+      }
+      prev = s;
+      if (++s == W_STAGES) { s = 0; sph ^= 1u; }
+    }
+    wgmma_wait<0>();
+    fence_regs(acc);
+    if (prev >= 0 && lane == 0) mbar_arrive(empty0 + 8 * prev);
+    store_tile<WBN>(p, epi, acc, m0, n0, m0 + rbase, q4, tmax);
+  }
+  if (p.amax_out) amax_commit(p.amax_out, tmax);     // one atomicMax per consumer warp per launch
+}
+
 }  // namespace tc
 
 // Host-visible tiling rule (mirrored by the Python packer mvector/engine.py::tc_tile_n).  The accumulator lives in the
@@ -575,6 +771,18 @@ bool conv_tc_supported(const ConvParams& p) {
   // gather composes both (common.cuh::gather_a4)
   if (p.pre_s != nullptr && p.src2_mode != VP_SRC2_NONE) return false;
   return true;
+}
+
+// persistent grids: one CTA per SM of the current device
+static int sm_count() {
+  int dev = 0, sms = 132;
+  cudaGetDevice(&dev);
+  static int count[64] = {};
+  if (dev >= 0 && dev < 64) {
+    if (count[dev] == 0) cudaDeviceGetAttribute(&count[dev], cudaDevAttrMultiProcessorCount, dev);
+    if (count[dev] > 0) sms = count[dev];
+  }
+  return sms;
 }
 
 // f16 = true: two-term FP16 split (conv_tc_kernel<0, true, BN>); w_img is then the fp16 weight image and descale the
@@ -599,13 +807,7 @@ static cudaError_t launch_conv_tc_impl(const ConvParams& p, const float* w_img, 
   static int debug_flags = -1;
   if (debug_flags < 0) { const char* e = getenv("VPB_TC_DEBUG"); debug_flags = e ? atoi(e) : 0; }
   a.debug = debug_flags;
-  int dev = 0, sms = 132;
-  cudaGetDevice(&dev);
-  static int sm_count[64] = {};
-  if (dev >= 0 && dev < 64) {
-    if (sm_count[dev] == 0) cudaDeviceGetAttribute(&sm_count[dev], cudaDevAttrMultiProcessorCount, dev);
-    if (sm_count[dev] > 0) sms = sm_count[dev];
-  }
+  const int sms = sm_count();
   const int groups = a.m_tiles * a.n_tiles;
   cudaLaunchConfig_t cfg{};
   cfg.gridDim = dim3(sms < groups ? sms : groups);
@@ -640,7 +842,76 @@ bool conv_tc16_supported(const ConvParams& p) {
   return p.N >= 128;                                  // narrow layers are not tensor bound: nothing to gain
 }
 
+// The wide path (conv_tc16_wide_kernel): a pointwise, stride-1, unpadded conv reading one plain source, unchunked, whose
+// A view [M, K] (base src + in_coff, row pitch in_ld) is a legal TMA tensor and whose N splits into 256-wide tiles.
+// N >= 1024 only: at N = 512 (ECAPA's tdnn1 / tdnn2, M = 76 288) the wide kernel measured 4 % slower than the 128-wide
+// one (9.03 waves of 256-wide tiles on 132 SMs against 19 of 128-wide ones), at N = 1536 it is faster.
+static bool tc16_wide_ok(const ConvParams& p) {
+  if (p.KT != 1 || p.KF != 1 || p.sT != 1 || p.sF != 1 || p.padT != 0 || p.padF != 0) return false;
+  if (p.Tin != p.Tout || p.Fin != p.Fout) return false;       // output row m reads source row m
+  if (p.src2_mode != VP_SRC2_NONE || p.tc_kc != 0) return false;
+  if (p.N % tc::WBN != 0 || p.N < 1024) return false;
+  if ((p.in_ld & 3) || (p.in_coff & 3) || (p.out_ld & 3) || (p.out_coff & 3)) return false;
+  return ((uintptr_t)(p.src + p.in_coff) & 15) == 0;
+}
+
+static PFN_cuTensorMapEncodeTiled_v12000 tensor_map_encoder() {
+  static PFN_cuTensorMapEncodeTiled_v12000 fn = nullptr;
+  if (fn == nullptr) {
+    void* f = nullptr;
+    cudaDriverEntryPointQueryResult q;
+    if (cudaGetDriverEntryPointByVersion("cuTensorMapEncodeTiled", &f, 12000, cudaEnableDefault, &q) == cudaSuccess &&
+        q == cudaDriverEntryPointSuccess)
+      fn = reinterpret_cast<PFN_cuTensorMapEncodeTiled_v12000>(f);
+  }
+  return fn;
+}
+
+static cudaError_t launch_conv_tc16_wide(const ConvParams& p, const float* w_tc16, float descale, cudaStream_t stream) {
+  using namespace tc;
+  PFN_cuTensorMapEncodeTiled_v12000 encode = tensor_map_encoder();
+  if (encode == nullptr) return cudaErrorNotSupported;
+  // A = the [M, K] fp32 view, boxes of 32 columns (128 B, one SWIZZLE_128B row) x 128 rows; reads outside it are zeros
+  CUtensorMap amap;
+  const cuuint64_t dims[2] = {(cuuint64_t)p.K, (cuuint64_t)p.M};
+  const cuuint64_t strides[1] = {(cuuint64_t)p.in_ld * 4u};
+  const cuuint32_t box[2] = {32u, (cuuint32_t)BM};
+  const cuuint32_t elem[2] = {1u, 1u};
+  if (encode(&amap, CU_TENSOR_MAP_DATA_TYPE_FLOAT32, 2, const_cast<float*>(p.src + p.in_coff), dims, strides, box, elem,
+             CU_TENSOR_MAP_INTERLEAVE_NONE, CU_TENSOR_MAP_SWIZZLE_128B, CU_TENSOR_MAP_L2_PROMOTION_L2_256B,
+             CU_TENSOR_MAP_FLOAT_OOB_FILL_NONE) != CUDA_SUCCESS)
+    return cudaErrorInvalidValue;
+  WideArgs a;
+  a.w_tc16 = reinterpret_cast<const uint8_t*>(w_tc16);
+  a.m_tiles = (p.M + BM - 1) / BM;
+  a.n_tiles = p.N / WBN;
+  a.k_blocks = (p.K + 63) / 64;
+  a.descale = descale;
+  const int groups = a.m_tiles * a.n_tiles;
+  const int sms = sm_count();
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(sms < groups ? sms : groups);
+  cfg.blockDim = dim3(W_THREADS);
+  cfg.dynamicSmemBytes = W_SMEM;
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled();
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  static PerDeviceSmem once;
+  if (once.need(cfg.dynamicSmemBytes)) {
+    cudaError_t e = cudaFuncSetAttribute(conv_tc16_wide_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, W_SMEM);
+    if (e != cudaSuccess) return e;
+    once.set(cfg.dynamicSmemBytes);
+  }
+  cudaError_t e = cudaLaunchKernelEx(&cfg, conv_tc16_wide_kernel, p, a, amap);
+  if (e != cudaSuccess) return e;
+  return cudaGetLastError();
+}
+
 cudaError_t launch_conv_tc16(const ConvParams& p, const float* w_tc16, float descale, cudaStream_t stream) {
+  if (tc16_wide_ok(p)) return launch_conv_tc16_wide(p, w_tc16, descale, stream);
   return launch_conv_tc_impl(p, w_tc16, true, descale, stream);
 }
 
