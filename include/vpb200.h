@@ -231,7 +231,9 @@ typedef struct vp_op {
   int32_t reserved0;
 } vp_op;
 
-/* Upload the packed fp32 weight arena (host pointer, copied to the device; replaces any previous arena). */
+/* Upload the packed fp32 weight arena (host pointer, copied to the device; replaces any previous arena).  Programs
+ * created before the call -- whether it succeeds or not -- are validated against the old arena: vp_embed,
+ * vp_embed_profiled and vp_embed_wave refuse them with VP_ERR_INVALID before launching anything. */
 int vp_weights_load(vp_handle* h, const void* host_blob, size_t nbytes);
 
 /* Validate + own a program for fixed (B, T).  Its workspace is the handle's shared arena, grown (after draining the

@@ -4,8 +4,9 @@ tests/test_op_edges_cpu.py on the CPU).
 A case is a dict.  ``build(case)`` lowers it into a one-op (or few-op) program with PlanBuilder / WeightArena: the op
 under test, the copies that feed it (a tracked workspace source for the fp16 split, gate / per-utterance-bias rows, an
 accumulate-into view, the columns around an output window) and, for the amax cases, a TC16 conv consuming its output.
-``run_gpu`` runs the program through Program.run_profiled; ``Sim(pb, blob, X).run()`` (tests/plan_sim.py) is the
-fp64 reference.
+``run_gpu`` runs the program eagerly, profiled, as a captured CUDA graph and as a replay of that graph on a second
+input, and requires the runs to agree bit for bit; ``Sim(pb, blob, X).run()`` (tests/plan_sim.py) is the fp64
+reference.
 
 Every case names the kernel it is meant to reach (``kernel``) and, for convs, the engine it requests (``engine``;
 'auto' expects the engine ``engine_of`` resolves); the GPU tests assert the engine from run_profiled, the CPU tests
@@ -347,8 +348,28 @@ def sim(b):
     return Sim(b.pb, b.blob, b.X).run().reshape(b.out_rows, b.out_cols)
 
 
-def run_gpu(b, runs=1):
+def second_input(X):
+    """The input the graph replay runs on: X with its rows reversed (same columns, same value ranges, other data)."""
+    return X[::-1].copy()
+
+
+def assert_bit_identical(runs):
+    """Every output of ``runs`` ({label: array}) equals the first one bit for bit (NaNs included)."""
+    (l0, a0), *rest = runs.items()
+    for label, a in rest:
+        bad = a.view(np.uint32) != a0.view(np.uint32)
+        assert not bad.any(), f'{label} != {l0}: {int(bad.sum())} elements differ, first at {np.argwhere(bad)[0]}'
+
+
+def run_gpu(b):
     """-> (output [out_rows, out_cols], the per-op run_profiled records).  The Engine is closed before returning.
+
+    One Program runs the case five times, on the same ``x`` / ``y`` tensors throughout (the CUDA graph is keyed on their
+    pointers): (1) Program.run, the first vp_embed, eager with PDL and no events; (2) run_profiled, eager with an event
+    before every op; (3) run, which captures the graph and launches it; then, with ``second_input(X)`` copied into x in
+    place, (4) run, a replay of that graph on new data, and (5) run_profiled.  The kernels are deterministic, so (1), (2)
+    and (3) must agree bit for bit, and (4) with (5): a graph that bakes in a value it should read at run time, a stale
+    pointer or an access that is wrong only under PDL overlap shows here.  (2) is returned.
 
     The output is NaN-poisoned before every run, as Sim poisons its own: consecutive cases often have the same shape
     and the same reference, and the caching allocator hands a case the block the previous case's result was just
@@ -361,11 +382,20 @@ def run_gpu(b, runs=1):
         prog = Program(eng, b.pb)
         y = torch.empty(b.out_rows, b.out_cols, device='cuda')
         x = torch.from_numpy(b.X).cuda().contiguous()
-        for _ in range(runs):
+        records = []
+
+        def once(run):
             y.fill_(float('nan'))
-            ops = prog.run_profiled(x, y)
-        torch.cuda.synchronize()
-        return y.cpu().numpy(), ops
+            records.append(run(x, y))
+            torch.cuda.synchronize()
+            return y.cpu().numpy()
+
+        first = dict(eager=once(prog.run), profiled=once(prog.run_profiled), captured=once(prog.run))
+        x.copy_(torch.from_numpy(second_input(b.X)))
+        second = dict(replayed=once(prog.run), profiled=once(prog.run_profiled))
+        assert_bit_identical(first)
+        assert_bit_identical(second)
+        return first['profiled'], records[1]
     finally:
         eng.close()
 
@@ -469,6 +499,31 @@ def engine_of(o, pref=None, tc16_on=None):
     return L.ENGINE_FFMA
 
 
+WIDE_BN = 256                                                       # conv_tc.cu tc::WBN
+
+
+def tc16_wide_ok(o):
+    """conv_tc.cu tc16_wide_ok: a pointwise, stride-1, unpadded, unchunked conv reading one plain source, N a multiple of
+    256 and >= 1024, ld / coff multiples of 4 and a 16-byte aligned A base.  The base is src + in_coff: workspace
+    buffers start on 256-byte boundaries (engine.ALIGN) and a TC16 op never reads the raw program input (it has no amax
+    slot), so the pointer condition is (4 * in_coff) % 16 == 0."""
+    return (o.KT == 1 and o.KF == 1 and o.sT == 1 and o.sF == 1 and o.padT == 0 and o.padF == 0
+            and o.Tin == o.Tout and o.Fin == o.Fout and o.src2_mode == L.SRC2_NONE and o.tc_kc == 0
+            and o.Cout % WIDE_BN == 0 and o.Cout >= 1024
+            and o.in_ld % 4 == 0 and o.in_coff % 4 == 0 and o.out_ld % 4 == 0 and o.out_coff % 4 == 0
+            and o.src >= 0 and o.src % 16 == 0 and (4 * o.in_coff) % 16 == 0)
+
+
+def wide_schedule(o):
+    """Tile schedule of conv_tc16_wide_kernel (launch_conv_tc16_wide): 128 x 256 tiles, 64-wide K blocks, a persistent
+    grid of min(SMs, tiles) CTAs; its TMA / weight stage ring has 2 stages (W_STAGES), carried across a CTA's tiles."""
+    K, M = o.KT * o.KF * o.Cin, o.B * o.Tout * o.Fout
+    m_tiles, n_tiles, k_blocks = (M + 127) // 128, o.Cout // WIDE_BN, (K + 63) // 64
+    tiles = m_tiles * n_tiles
+    return dict(M=M, K=K, m_tiles=m_tiles, n_tiles=n_tiles, tiles=tiles, tiles_per_cta=-(-tiles // min(SMS, tiles)),
+                k_blocks=k_blocks, k_tail=K % 64, m_tail=M % 128)
+
+
 def _tc_suffix(pre, add):
     """conv_tc.cu:621-624: the prologue selects conv_tc_kernel<2, ...>, else an added second source <1, ...>, else <0>."""
     return ',pre' if pre else ',add' if add else ''
@@ -480,7 +535,7 @@ def kernel_of(o, engine):
         return 'conv_c1_wide' if c1_wide(o) else 'conv_c1'
     if o.kind == L.OP_CONV:
         if engine == L.ENGINE_TC16:
-            return 'conv_tc<f16>'
+            return 'conv_tc16_wide' if tc16_wide_ok(o) else 'conv_tc<f16>'
         if engine == L.ENGINE_TC:
             return 'conv_tc<tf32%s>' % _tc_suffix(o.pre_s >= 0, o.src2_mode == L.SRC2_ADD)
         if small_m_ok(o):
@@ -707,6 +762,7 @@ for _name, _c in dict(
         k_tail_72=dict(seed=14, B=11, Tin=100, Cin=24, N=24, KT=3, padT=1, bias=True, act=L.ACT_HARDTANH20),
 ).items():
     _tc(_name, ('ffma', 'tc', 'tc16') if _name in _TC16_GEOMETRIES else ('ffma', 'tc'), table=ENGINE_CASES, **_c)
+ENGINE_CASES['gemm_n1536_k128-tc16']['kernel'] = 'conv_tc16_wide'     # pointwise, N = 1536: the wide path
 
 # ---- engine routing: what AUTO resolves to where a tensor-core engine cannot take the op, and the explicit requests
 # vp_program_create refuses (VP_ERR_UNSUPPORTED; engine_of raises ValueError) rather than run differently ----
@@ -849,10 +905,11 @@ AMAX_WRITERS = dict(
     ffma_conv=dict(op='conv', engine='ffma', B=4, Tin=300, Cin=64, N=64, KT=3, padT=1, bias=True, out_C=64),
     tf32_conv=dict(op='conv', engine='tc', B=4, Tin=300, Cin=64, N=64, KT=3, padT=1, bias=True, out_C=64),
     tc16_conv=dict(op='conv', engine='tc16', B=4, Tin=300, Cin=64, N=128, KT=3, padT=1, bias=True, out_C=128),
+    tc16_wide_conv=dict(op='conv', engine='tc16', B=4, Tin=300, Cin=64, N=1024, bias=True, out_C=1024),
 )
 AMAX_KERNELS = dict(ew_gate_res='ew', ew_aff='ew', pad_copy='pad_copy', pool2d='pool2d', c1_wide='conv_c1_wide',
                     c1_generic='conv_c1', ffma_conv='conv_ffma<64>', tf32_conv='conv_tc<tf32>',
-                    tc16_conv='conv_tc<f16>', small_m_1024='linear_small_m')
+                    tc16_conv='conv_tc<f16>', tc16_wide_conv='conv_tc16_wide', small_m_1024='linear_small_m')
 RANGE_SCALES = (1e-30, 1e-6, 1e6, 1e30)
 # the scale multiplies every input AND the writers' biases, so the tensor the consumer reads is O(scale) at both ends
 # of the sweep (an unscaled bias of ~0.1 would run the small-scale half at unit scale)
@@ -883,3 +940,53 @@ GRAPH_RESET = dict(op='ew', mode='COPY', B=4, T=300, C=64, out_C=64, seed=440, k
 TC16_RANGE_CASES = {f'gemm_512-{_s:g}': dict(op='ew', mode='COPY', B=8, T=298, C=512, out_C=512, seed=450, scale=_s,
                                              kernel='ew', consumer=dict(B=8, T=298, N=512))
                     for _s in (1e-30, 1e-8, 1e-3, 1e4, 1e9, 1e30)}
+
+# ---- the fp16 split's wide path (conv_tc16_wide_kernel, tests/test_gpu_tc16_wide.py): 128 x 256 tiles for pointwise,
+# stride-1, unpadded, unchunked convs with one plain source and N % 256 == 0, N >= 1024 (tc16_wide_ok).  Its edges, and
+# the convs just outside the predicate, which stay on the 128-wide kernel ----
+TC16_WIDE_CASES = {}
+
+
+def _wide(name, seed, kernel='conv_tc16_wide', **c):
+    TC16_WIDE_CASES[name] = dict(op='conv', engine='tc16', kernel=kernel, seed=seed, **c)
+
+
+_wide('m_tail', 201, B=3, Tin=683, Cin=512, N=1024, bias=True, act=L.ACT_RELU, intent=dict(m_tail=1))
+_wide('k_tail', 202, B=2, Tin=700, Cin=72, N=1024, bias=True, intent=dict(k_blocks=2, k_tail=8))
+_wide('k_tail_136', 203, B=2, Tin=700, Cin=136, N=1280, bias=True, act=L.ACT_RELU)
+_wide('in_window', 204, B=4, Tin=300, Cin=512, in_coff=1024, N=1536, bias=True)          # cat slice, in_ld 1536
+_wide('out_window', 205, B=4, Tin=300, Cin=128, N=1024, out_coff=516, bias=True, act=L.ACT_RELU)
+_wide('relu_bn_res', 206, B=4, Tin=300, Cin=512, N=1536, bias=True, act=L.ACT_RELU, post=True, res=True)
+_wide('res_act2_tail', 207, B=3, Tin=683, Cin=128, N=1024, bias=True, res=True, act2=L.ACT_RELU)
+_wide('tiles_4', 208, B=1, Tin=1024, Cin=256, N=1024, bias=True, intent=dict(tiles=32))    # 8 x 4 tiles on 32 CTAs
+_wide('tiles_152', 209, B=8, Tin=300, Cin=128, N=2048, bias=True, act=L.ACT_RELU,
+      intent=dict(tiles=152, tiles_per_cta=2, k_blocks=2))                                  # 19 x 8 on 132 CTAs
+_wide('general_epilogue', 210, B=4, Tin=300, Cin=128, N=1024, bias=True, ubias=True, act=L.ACT_SILU)
+_wide('scale_1e-30', 211, B=4, Tin=300, Cin=512, N=1024, bias=True, bias_scale=1e-30, scale=1e-30)
+_wide('scale_1e+30', 212, B=4, Tin=300, Cin=512, N=1024, bias=True, bias_scale=1e30, scale=1e30)
+# several tiles per CTA with an odd K-block count: the 2-stage ring's stage index and phase carry over from one tile to
+# the next on the other parity, and the next tile's residual is prefetched; 63 x 4 tiles with a 64-row M tail
+_wide('multi_tile_odd_k', 213, B=8, Tin=1000, Cin=192, N=1024, bias=True, act=L.ACT_RELU, res=True,
+      intent=dict(tiles=252, tiles_per_cta=2, k_blocks=3, m_tail=64))
+# 19 x 7 = 133 tiles on 132 CTAs: one CTA runs a second tile, 5 K blocks
+_wide('tiles_133', 214, B=8, Tin=304, Cin=320, N=1792, bias=True, act=L.ACT_RELU, post=True,
+      intent=dict(tiles=133, tiles_per_cta=2, k_blocks=5))
+# one partial K block (K < 64: the second 32-column TMA box lies wholly outside the tensor) and exactly one full one
+_wide('k8_one_partial_block', 215, B=4, Tin=300, Cin=8, N=1024, bias=True, intent=dict(k_blocks=1, k_tail=8))
+_wide('k40_one_partial_block', 216, B=4, Tin=300, Cin=40, N=1024, bias=True, act=L.ACT_RELU,
+      intent=dict(k_blocks=1, k_tail=40))
+_wide('k64_one_block', 217, B=4, Tin=300, Cin=64, N=1024, bias=True, intent=dict(k_blocks=1, k_tail=0))
+# the smallest M the tensor-core engines take, over four utterances
+_wide('m1024', 218, B=4, Tin=256, Cin=128, N=1280, bias=True, post=True, intent=dict(M=1024, m_tail=0))
+# the general epilogues of the 128-wide rows (gate_seg, sum_into, sigmoid_act2, tanh_act2_res) at N >= 1024
+_wide('gate_seg', 219, B=6, Tin=249, Cin=128, N=1024, gate=True, seg_len=100, n_seg=3)
+_wide('sum_into', 220, B=4, Tin=300, Cin=64, N=1024, bias=True, act=L.ACT_RELU, post=True, sum=True)
+_wide('sigmoid_act2', 221, B=4, Tin=300, Cin=64, N=1024, bias=True, post=True, act2=L.ACT_SIGMOID)
+_wide('tanh_act2_res', 222, B=4, Tin=300, Cin=64, N=1280, bias=True, res=True, act2=L.ACT_TANH)
+# just outside the predicate: N < 1024, N % 256 != 0, chunked accumulation, taps, a second source
+_NARROW = 'conv_tc<f16>'
+_wide('n512', 305, _NARROW, B=4, Tin=300, Cin=512, N=512, bias=True, act=L.ACT_RELU, post=True)
+_wide('n1152', 301, _NARROW, B=4, Tin=300, Cin=512, N=1152, bias=True, act=L.ACT_RELU)
+_wide('chunked_k2048', 302, _NARROW, B=4, Tin=300, Cin=2048, N=1024, bias=True)                   # tc_kc > 0
+_wide('k3_taps', 303, _NARROW, B=4, Tin=300, Cin=128, N=512, KT=3, padT=1, bias=True, act=L.ACT_RELU)
+_wide('concat', 304, _NARROW, B=4, Tin=300, Cin=128, Cin2=128, src2_mode=L.SRC2_CONCAT, N=1024, bias=True)

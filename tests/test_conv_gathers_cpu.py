@@ -2,7 +2,8 @@
 configurations reach, no GPU needed:
 
 * every tensor-core kernel instantiation (family, N tile, chunked or not) that a bench.py configuration runs -- on the
-  engines op_cases.engine_of resolves, with the fp16 split on and off -- is among the schedules of TC_CASES, so a model
+  engines op_cases.engine_of resolves, with the fp16 split on and off -- is among the schedules of TC_CASES and
+  TC16_WIDE_CASES, so a model
   change that reaches a new instantiation fails here until a case covers it;
 * the add and prologue families each reach the schedules and geometries their gathers branch on;
 * the MODE 0 twins the GPU compares against are what they claim to be."""
@@ -41,6 +42,9 @@ def test_product_tensor_core_kernels_are_covered(cfg):
     model, c = oc.bench_model(cfg)
     pb = model.lower(c['per_gpu'], oc.BENCH_T[cfg]).finalize()
     have = {_reach(o, oc.ENGINES[c['engine']]) for c, o, _, _ in _tc_cases().values()}
+    for case in oc.TC16_WIDE_CASES.values():                  # the fp16 split's wide path (conv_tc16_wide)
+        b = oc.build(case)
+        have.add(_reach(b.pb.ops[b.main], b.expect[b.main]))
     reach = set()
     for tc16_on in (True, False):
         for o in pb.ops:

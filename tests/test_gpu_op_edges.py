@@ -7,10 +7,15 @@ on both sides of their shared-memory limits) and the amax tracking that keeps th
 Each case is one op (plus the copies that feed it) from tests/op_cases.py, compared with the fp64 interpreter
 (tests/plan_sim.py).  Gates: FFMA kernels 2e-5 relative to max(1, max|ref|); split TF32 / fp16 split 1e-4; max pooling
 and copies bit-exact.  Every conv asserts the engine it ran on, so a case cannot pass through a silent fallback, and an
-engine request the op cannot take must be refused when the program is created.
+engine request the op cannot take must be refused when the program is created.  Every case also runs as a captured
+CUDA graph and as a replay of it on a second input (op_cases.run_gpu), bit-identical to the eager runs.
 
-The errors quoted in the docstrings were measured on an H100 80GB HBM3 at 700 W; the whole module runs in about 50 s
-there."""
+The program lifecycle tests at the end cover what the graph cache is keyed on: new input / output pointers, the
+fall-back to eager runs after 16 misses, an arena reallocated under a captured graph, a weight reload (programs created
+before it are refused) and two models sharing one Engine.
+
+The errors quoted in the docstrings were measured on an H100 80GB HBM3 at 700 W; this module, test_gpu_tc16_wide.py and
+test_gpu_conv_gathers.py run in about 80 s together there, every case five times."""
 import numpy as np
 import pytest
 import torch
@@ -140,7 +145,8 @@ def test_amax_writer_feeds_tc16(name):
     consumer too large a scale, and its fp16 hi terms overflow at any magnitude; a writer that reports nothing leaves
     the slot at 0, which means scale 1: overflow at the large scales, flush to zero at the small ones.  (Too large a
     maximum -- an over-reporting writer, a stale slot -- flushes small tensors to zero; see the graph-replay test.)
-    Measured max-rel error <= 1.7e-6 (2.3e-6 on the 512 x 512 GEMM)."""
+    Measured max-rel error <= 1.7e-6 (2.3e-6 on the 512 x 512 GEMM, 4.8e-6 behind the wide fp16-split writer, whose
+    consumer reduces over K = 1024)."""
     case = SCALED[name]
     b, got, ref = _run(case)
     assert b.pb.ops[b.consumer].amax_in > 0
@@ -186,3 +192,159 @@ def test_amax_slots_reset_between_graph_replays():
     assert np.isfinite(outs[1]).all() and np.isfinite(outs[2]).all()
     assert _rel(outs[1], ref, floor=0.0) <= 2e-5
     assert np.array_equal(outs[1].view(np.uint32), outs[2].view(np.uint32))
+
+
+# ---- program lifecycle: the graph cache keyed on (feats, emb, arena), its give-up path, arena growth, weight reloads ----
+def _profiled(prog, x, y):
+    """Eager run with per-op events (never a graph) -> output on the host."""
+    y.fill_(float('nan'))
+    prog.run_profiled(x, y)
+    return y.cpu().numpy()
+
+
+def _graphed(prog, x, y):
+    y.fill_(float('nan'))
+    prog.run(x, y)
+    torch.cuda.synchronize()
+    return y.cpu().numpy()
+
+
+def _same(got, want, what):
+    bad = got.view(np.uint32) != want.view(np.uint32)
+    assert not bad.any(), f'{what}: {int(bad.sum())} elements differ'
+
+
+LIFECYCLE = oc.TC_CASES['res_tail-tc16']          # copy -> TC16 conv with residual: an amax slot and the arena
+
+
+def test_graph_follows_new_pointers():
+    """Two inputs and two outputs alternated on one program: every (x, y) pair the graph was not captured for is
+    captured anew, and each result equals the eager run on that input bit for bit."""
+    from mvector.engine import Engine, Program
+    b = oc.build(LIFECYCLE)
+    eng = Engine()
+    try:
+        eng.load_weights(b.blob)
+        prog = Program(eng, b.pb)
+        xs = [torch.from_numpy(X).cuda() for X in (b.X, oc.second_input(b.X))]
+        ys = [torch.empty(b.out_rows, b.out_cols, device='cuda') for _ in range(2)]
+        want = [_profiled(prog, x, ys[0]) for x in xs]
+        for step in range(10):                    # (x0, y0), (x1, y0), (x0, y1), (x1, y1), ... each pair twice
+            i, j = step % 2, (step // 2) % 2
+            _same(_graphed(prog, xs[i], ys[j]), want[i], f'step {step}: x{i} -> y{j}')
+    finally:
+        eng.close()
+
+
+def test_graph_capture_given_up_after_16_misses():
+    """18 distinct (x, y) pairs, all alive, cycled twice: after 16 graph misses the program stops re-capturing and runs
+    eagerly (api.cu embed_graph); every result equals the eager run on its input."""
+    from mvector.engine import Engine, Program
+    b = oc.build(LIFECYCLE)
+    eng = Engine()
+    try:
+        eng.load_weights(b.blob)
+        prog = Program(eng, b.pb)
+        xs = [torch.from_numpy(np.ascontiguousarray(np.roll(b.X, 7 * k, axis=0))).cuda() for k in range(18)]
+        ys = [torch.empty(b.out_rows, b.out_cols, device='cuda') for _ in range(18)]
+        want = [_profiled(prog, x, ys[0]) for x in xs]
+        for rnd in range(2):
+            for k in range(18):
+                _same(_graphed(prog, xs[k], ys[k]), want[k], f'round {rnd}, pair {k}')
+    finally:
+        eng.close()
+
+
+def test_graph_recaptured_after_arena_growth():
+    """Program A is captured; program B (the same weights at ten times the batch) needs a larger workspace, so the
+    handle's arena is reallocated; A's graph holds the freed arena and must be re-captured.  A, B, A each equal their
+    eager results."""
+    from mvector.engine import Engine, Program
+    a, big = oc.build(LIFECYCLE), oc.build(oc.with_batch(LIFECYCLE, 40))
+    np.testing.assert_array_equal(a.blob, big.blob)
+    eng = Engine()
+    try:
+        eng.load_weights(a.blob)
+        pa = Program(eng, a.pb)
+        xa, ya = torch.from_numpy(a.X).cuda(), torch.empty(a.out_rows, a.out_cols, device='cuda')
+        want_a = _profiled(pa, xa, ya)
+        _graphed(pa, xa, ya)                                           # eager
+        _same(_graphed(pa, xa, ya), want_a, 'A captured')
+        arena = L.lib().vp_workspace_bytes(eng.handle)
+        pbig = Program(eng, big.pb)
+        assert L.lib().vp_workspace_bytes(eng.handle) > arena
+        xb, yb = torch.from_numpy(big.X).cuda(), torch.empty(big.out_rows, big.out_cols, device='cuda')
+        want_b = _profiled(pbig, xb, yb)
+        _graphed(pbig, xb, yb)                                         # B's eager first run
+        _same(_graphed(pa, xa, ya), want_a, 'A after the arena grew')
+        _same(_graphed(pbig, xb, yb), want_b, 'B captured')
+        _same(_graphed(pa, xa, ya), want_a, 'A replayed')
+    finally:
+        eng.close()
+    assert _rel(want_a, oc.sim(a)) <= 1e-4
+
+
+def test_programs_refused_after_weight_reload():
+    """A program validated against one weights blob is refused once another is loaded -- run, run_profiled and
+    run_wave raise VP_ERR_INVALID before anything is launched (the output stays NaN) -- rather than replay a graph
+    that reads the freed blob with the old blob's offsets and fp16 descales.  A program created after the reload runs
+    on the new blob."""
+    from mvector.engine import Engine, Program
+    old, new = oc.build(LIFECYCLE), oc.build(dict(oc.GRAPH_RESET))
+    assert new.blob.nbytes < old.blob.nbytes                          # the old offsets would overrun the new blob
+    eng = Engine()
+    try:
+        eng.load_weights(old.blob)
+        prog = Program(eng, old.pb)
+        x, y = torch.from_numpy(old.X).cuda(), torch.empty(old.out_rows, old.out_cols, device='cuda')
+        _graphed(prog, x, y)
+        _graphed(prog, x, y)                                           # captured
+        eng.load_weights(new.blob)
+        wave = torch.zeros(4, 16000, device='cuda')
+        for what, call in (('run', lambda: prog.run(x, y)), ('run_profiled', lambda: prog.run_profiled(x, y)),
+                           ('run_wave', lambda: prog.run_wave(wave, None, x, x, y))):
+            y.fill_(float('nan'))
+            with pytest.raises(L.VpError) as e:
+                call()
+            assert e.value.code == L.VP_ERR_INVALID, (what, e.value)
+            torch.cuda.synchronize()
+            assert torch.isnan(y).all(), what
+        fresh = Program(eng, new.pb)
+        xn, yn = torch.from_numpy(new.X).cuda(), torch.empty(new.out_rows, new.out_cols, device='cuda')
+        got = [_graphed(fresh, xn, yn) for _ in range(3)]             # eager, captured, replayed
+        _same(got[1], got[0], 'captured')
+        _same(got[2], got[0], 'replayed')
+    finally:
+        eng.close()
+    assert _rel(got[0], oc.sim(new), floor=0.0) <= 2e-5
+
+
+def test_models_sharing_an_engine(manifest):
+    """Two models on one Engine (load_state_dict(..., engine=e)) called alternately: each re-uploads its own blob when
+    the other's is resident, and every output equals the same model on a private Engine bit for bit."""
+    from conftest import load_golden
+    from mvector.engine import Engine
+    from mvector.models import build_model
+    from mvector.utils.utils import dict_to_object
+
+    def model(name, engine=None):
+        m, (_, sd) = manifest[name], load_golden(name)
+        net = build_model(m['feature_dim'], dict_to_object({'model_conf': {'model': m['model'],
+                                                                            'model_args': m['model_args']}}))
+        net.load_state_dict({'0.' + k: v for k, v in sd.items()}, engine=engine)
+        return net
+
+    names = ('tdnn_small', 'ecapa_small')
+    feats = {n: torch.from_numpy(load_golden(n)[0]['feats']).cuda().float().contiguous() for n in names}
+    private = {n: model(n) for n in names}
+    want = {n: private[n](feats[n]).cpu().numpy() for n in names}
+    e = Engine()
+    try:
+        shared = {n: model(n, engine=e) for n in names}
+        for step in range(6):
+            n = names[step % 2]
+            _same(shared[n](feats[n]).cpu().numpy(), want[n], f'step {step}: {n}')
+    finally:
+        e.close()
+        for m in private.values():
+            m.engine.close()

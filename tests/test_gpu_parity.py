@@ -178,13 +178,24 @@ SMALL = ['ecapa_small', 'tdnn_small', 'campplus_small', 'resnetse_small', 'eres2
 
 @pytest.mark.parametrize('name', SMALL)
 def test_small_models_vs_reference_golden(name, manifest):
-    """Backbone from the reference's golden FEATURES -> embedding, and waveform -> embedding through the fused path."""
+    """Backbone from the reference's golden FEATURES -> embedding, and waveform -> embedding through the fused path.
+    The program runs three times on the same input and output tensors -- eager, captured as a CUDA graph, replayed --
+    with bit-identical embeddings."""
     from plan_sim import simulate
     m = manifest[name]
     z, sd = load_golden(name)
     model = _model(m['model'], m['feature_dim'], m['model_args'], sd)
-    feats = torch.from_numpy(z['feats']).cuda()
-    emb = model(feats).cpu().numpy()
+    feats = torch.from_numpy(z['feats']).cuda().float().contiguous()
+    prog = model.program(feats.shape[0], feats.shape[1])
+    y = torch.empty(feats.shape[0], model.embd_dim, device='cuda')
+    runs = []
+    for _ in range(3):
+        y.fill_(float('nan'))
+        prog.run(feats, y)
+        runs.append(y.cpu().numpy())
+    for label, r in zip(('captured', 'replayed'), runs[1:]):
+        assert np.array_equal(r.view(np.uint32), runs[0].view(np.uint32)), label
+    emb = runs[0]
     assert rel_l2(emb, z['emb']).max() < EMB_TOL
     sim, _ = simulate(model, z['feats'])
     assert rel_l2(emb, sim).max() < EMB_TOL

@@ -20,7 +20,8 @@ ALL = {**{f'tc/{k}': v for k, v in oc.TC_CASES.items()}, **{f'engine/{k}': v for
        **{f'ffma/{k}': v for k, v in oc.FFMA_CASES.items()},
        **{f'glue/{k}': v for k, v in oc.GLUE_CASES.items()}, **{f'amax/{k}': v for k, v in oc.AMAX_CASES.items()},
        **{f'shared/{k}': v for k, v in oc.SHARED_SLOT_CASES.items()}, 'graph/reset': oc.GRAPH_RESET,
-       **{f'range/{k}': v for k, v in oc.TC16_RANGE_CASES.items()}}
+       **{f'range/{k}': v for k, v in oc.TC16_RANGE_CASES.items()},
+       **{f'wide/{k}': v for k, v in oc.TC16_WIDE_CASES.items()}}
 SCALED = {**oc.AMAX_CASES, **oc.TC16_RANGE_CASES}
 
 
@@ -253,6 +254,45 @@ def test_tc_coverage():
     assert k2304 == {'tc': 8, 'tc16': 4}, k2304
 
 
+def _wide_schedules():
+    out = {}
+    for name, case in oc.TC16_WIDE_CASES.items():
+        if case['kernel'] == 'conv_tc16_wide':
+            b = oc.build(case)
+            out[name] = (case, b.pb.ops[b.main], oc.wide_schedule(b.pb.ops[b.main]))
+    return out
+
+
+def test_tc16_wide_cases_have_the_schedules_they_claim():
+    for name, (case, _, s) in _wide_schedules().items():
+        for key, want in case.get('intent', {}).items():
+            assert s[key] == want, (name, key, s)
+
+
+def test_tc16_wide_coverage():
+    """The wide kernel's edges: several tiles per CTA with an odd K-block count and a residual (the 2-stage ring's
+    phase carried across tiles, the next tile's residual prefetched), exactly 133 tiles, an M tail of one row, K < 64
+    in one partial block, K = 64 in one full block, a K tail after full blocks, M = 1024, input and output column
+    windows, and every epilogue feature (residual, affine, ubias, per-segment gate, accumulate-into, SiLU / sigmoid /
+    tanh)."""
+    W = {n: (o, s) for n, (_, o, s) in _wide_schedules().items()}
+    sched = [s for _, s in W.values()]
+    assert any(s['tiles_per_cta'] >= 2 and s['k_blocks'] % 2 == 1 and s['k_blocks'] > 1 and o.res != L.BUF_NONE
+               for o, s in W.values())
+    assert any(s['tiles'] == 133 and s['tiles_per_cta'] == 2 for s in sched)
+    assert any(s['m_tail'] == 1 for s in sched)
+    assert {8, 40} <= {s['K'] for s in sched if s['k_blocks'] == 1 and s['k_tail']}
+    assert any(s['K'] == 64 for s in sched)
+    assert any(s['k_blocks'] > 1 and s['k_tail'] for s in sched)
+    assert min(s['M'] for s in sched) == 1024
+    ops = [o for o, _ in W.values()]
+    assert any(o.in_coff > 0 for o in ops) and any(o.out_coff > 0 for o in ops)
+    assert any(o.gate != L.BUF_NONE and o.n_seg > 1 for o in ops)
+    assert any(o.ubias != L.BUF_NONE for o in ops) and any(o.sum != L.BUF_NONE for o in ops)
+    assert any(o.post_s >= 0 for o in ops) and any(o.res != L.BUF_NONE for o in ops)
+    assert {L.ACT_SILU, L.ACT_SIGMOID, L.ACT_TANH} <= {o.act for o in ops} | {o.act2 for o in ops}
+
+
 def test_position_invariance_case_lands_on_full_and_tail_tiles():
     for variant, engine in ((v, e) for v in oc.INVARIANCE_VARIANTS for e in ('tc', 'ffma')):
         b16 = oc.build(oc.invariance(variant, engine, 16))
@@ -272,8 +312,9 @@ def test_every_kernel_is_reached():
     for case in ALL.values():
         b = oc.build(_small(case))
         reached |= {_kernel(b, i) for i in _main_ops(b)}
-    want = {'conv_tc<tf32>', 'conv_tc<tf32,add>', 'conv_tc<tf32,pre>', 'conv_tc<f16>', 'conv_ffma<32>', 'conv_ffma<64>',
-            'conv_ffma<128>', 'linear_small_m', 'conv_c1_wide', 'conv_c1', 'pool2d', 'ew', 'pad_copy', 'colstats', 'colstats_smem', 'asp', 'asp_smem'}
+    want = {'conv_tc<tf32>', 'conv_tc<tf32,add>', 'conv_tc<tf32,pre>', 'conv_tc<f16>', 'conv_tc16_wide', 'conv_ffma<32>',
+            'conv_ffma<64>', 'conv_ffma<128>', 'linear_small_m', 'conv_c1_wide', 'conv_c1', 'pool2d', 'ew', 'pad_copy',
+            'colstats', 'colstats_smem', 'asp', 'asp_smem'}
     assert want <= reached, want - reached
 
 
@@ -332,7 +373,7 @@ def test_amax_consumer_sees_the_scale(name):
 def test_amax_writers_cover_every_writer_kernel():
     kernels = {oc.AMAX_KERNELS[n.split('-')[0]] for n in oc.AMAX_CASES}
     assert kernels == {'ew', 'pad_copy', 'pool2d', 'conv_c1_wide', 'conv_c1', 'conv_ffma<64>', 'linear_small_m',
-                       'conv_tc<tf32>', 'conv_tc<f16>'}
+                       'conv_tc<tf32>', 'conv_tc<f16>', 'conv_tc16_wide'}
     scales = {c['scale'] for c in oc.AMAX_CASES.values()}
     assert scales == set(oc.RANGE_SCALES)
     b = oc.build(oc.AMAX_CASES['small_m_1024-1e+06'])

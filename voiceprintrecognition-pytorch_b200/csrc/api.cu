@@ -19,6 +19,9 @@ struct vp_handle {
   // weights
   float* d_weights = nullptr;
   size_t weights_bytes = 0;
+  // bumped by every vp_weights_load, failed or not: a program validated against an older blob (its weight offsets and
+  // extents, its fp16 images' descale) must not run against the new one, nor its graph read the freed allocation
+  int weights_gen = 0;
   // ONE workspace arena shared by all programs of the handle (a handle runs one program at a time, stream-ordered):
   // sized to the largest live program, so serving ragged lengths costs max(ws), not sum(ws), of device memory
   char* d_arena = nullptr;
@@ -53,6 +56,7 @@ struct vp_program {
   int runs = 0, g_miss = 0;
   bool g_off = false;
   int n_slots = 0;            // amax slots (uint32 each) behind the workspace, zeroed at the start of every run
+  int weights_gen = 0;        // the handle's weights_gen the program was validated against
   size_t arena_need() const { return ws_bytes + (((size_t)n_slots * 4 + 255) & ~(size_t)255); }
   unsigned* slot(int32_t q) const { return q > 0 ? reinterpret_cast<unsigned*>(h->d_arena + ws_bytes) + (q - 1) : nullptr; }
 };
@@ -351,8 +355,10 @@ int vp_mfcc_finish(vp_handle* h, int32_t B, int32_t Lpad, const int32_t* keep, f
 int vp_weights_load(vp_handle* h, const void* blob, size_t nbytes) {
   if (!h || !blob || nbytes == 0 || (nbytes & 15)) return fail(h, VP_ERR_INVALID, "weights blob must be non-empty, 16 B multiple");
   CUDA_TRY(h, cudaSetDevice(h->device));
+  ++h->weights_gen;           // before the old blob is freed: every existing program is stale from here, load or no load
   cudaFree(h->d_weights);
   h->d_weights = nullptr;
+  h->weights_bytes = 0;
   CUDA_TRY(h, cudaMalloc(&h->d_weights, nbytes));
   CUDA_TRY(h, cudaMemcpy(h->d_weights, blob, nbytes, cudaMemcpyHostToDevice));
   h->weights_bytes = nbytes;
@@ -537,6 +543,7 @@ int vp_program_create(vp_handle* h, const vp_op* ops, int32_t n_ops, size_t ws_b
   vp_program* p = new (std::nothrow) vp_program();
   if (!p) return fail(h, VP_ERR_NOMEM, "host alloc");
   p->h = h;
+  p->weights_gen = h->weights_gen;
   p->ops.assign(ops, ops + n_ops);
   p->ws_bytes = (ws_bytes + 255) & ~(size_t)255;
   p->in_floats = in_floats;
@@ -761,8 +768,16 @@ static int embed_graph(vp_program* p, const float* feats, float* emb, cudaStream
   return VP_OK;
 }
 
+// A program is lowered and validated against one weights blob; after vp_weights_load it is refused, not re-captured: its
+// offsets, extents and fp16 descales belong to the old blob.
+static int check_weights_gen(const vp_program* p) {
+  if (p->weights_gen == p->h->weights_gen) return VP_OK;
+  return fail(p->h, VP_ERR_INVALID, "program was created before the weights were reloaded: create it again");
+}
+
 int vp_embed(vp_program* p, const float* feats, float* emb, void* stream) {
   if (!p || !feats || !emb) return p ? fail(p->h, VP_ERR_INVALID, "null argument") : VP_ERR_INVALID;
+  TRY(check_weights_gen(p));
   CUDA_TRY(p->h, cudaSetDevice(p->h->device));
   if (p->g_off || p->runs++ == 0) return run_ops(p, feats, emb, (cudaStream_t)stream, nullptr);
   return embed_graph(p, feats, emb, (cudaStream_t)stream);
@@ -770,6 +785,7 @@ int vp_embed(vp_program* p, const float* feats, float* emb, void* stream) {
 
 int vp_embed_profiled(vp_program* p, const float* feats, float* emb, void* stream, float* ms_per_op) {
   if (!p || !feats || !emb || !ms_per_op) return p ? fail(p->h, VP_ERR_INVALID, "null argument") : VP_ERR_INVALID;
+  TRY(check_weights_gen(p));
   vp_handle* h = p->h;
   const size_t n = p->ops.size();
   std::vector<cudaEvent_t> evs(n + 1);
@@ -807,6 +823,7 @@ int vp_embed_wave(vp_program* p, const float* wave, int32_t B, int32_t Lpad, con
   if (!p) return VP_ERR_INVALID;
   // check the call against the program BEFORE anything is launched: the front-end writes B*T*F floats into
   // feats_scratch, which a host sizes from the program
+  TRY(check_weights_gen(p));
   if (!p->h->fe_set) return fail(p->h, VP_ERR_INVALID, "front-end not configured (vp_frontend_set)");
   const int T = vp_num_frames(p->h, Lpad);
   if (B < 1 || T < 1) return fail(p->h, VP_ERR_INVALID, "empty batch / waveform shorter than one frame");

@@ -35,6 +35,7 @@ class Engine:
         if rc != L.VP_OK:
             raise L.VpError(rc, 'vp_create failed (needs an sm_90 GPU: H100)')
         self._programs = []
+        self.weights_owner = None       # which caller's blob the handle holds (load_weights(owner=...))
 
     @property
     def handle(self):
@@ -43,9 +44,14 @@ class Engine:
     def stream_ptr(self):
         return C.c_void_p(torch.cuda.current_stream(self.device).cuda_stream)
 
-    def load_weights(self, blob):
+    def load_weights(self, blob, owner=None):
+        """Upload a weight blob, replacing the previous one: every Program created before it is refused from then on
+        (vp_weights_load).  ``owner`` records whose blob the handle now holds, so models sharing one Engine can tell
+        whether theirs is still resident (Backbone.program)."""
         blob = np.ascontiguousarray(blob, dtype=np.float32)
+        self.weights_owner = None
         _check(self._h, L.lib().vp_weights_load(self._h, blob.ctypes.data_as(C.c_void_p), blob.nbytes))
+        self.weights_owner = owner
 
     def cosine_scores(self, a, b):
         """[n, D] x [m, D] -> device tensor [n, m] of cosine similarities (vp_cosine_scores); inputs: numpy / torch."""

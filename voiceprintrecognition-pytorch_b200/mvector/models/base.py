@@ -69,7 +69,7 @@ class Backbone:
         self.max_cached_programs = 64      # programs are host-side op lists: the workspace is the handle's shared arena
         self.training = False
         self._blob = None
-        self._uploaded = False
+        self._blob_id = None               # identifies this blob on an Engine (Engine.weights_owner)
 
     # -- nn.Module-ish surface used by the reference's call sites (predict.py:55-63) --
     def eval(self):
@@ -106,7 +106,7 @@ class Backbone:
         self._off = {}
         self._pack(sd, arena)
         self._blob = arena.blob()          # uploaded lazily: ingesting weights / lowering needs no GPU
-        self._uploaded = False
+        self._blob_id = object()
         self._arena_index = arena.index
         for p in self._programs.values():
             p.close()
@@ -122,14 +122,18 @@ class Backbone:
         return pb
 
     def program(self, B, T):
+        if self.engine is None:
+            self.engine = Engine()
+        if self.engine.weights_owner is not self._blob_id:
+            # not uploaded yet, or another model sharing the Engine has uploaded its blob since: the handle refuses
+            # every program created before that reload, so drop them and upload ours again
+            for p in self._programs.values():
+                p.close()
+            self._programs.clear()
+            self.engine.load_weights(self._blob, owner=self._blob_id)
         key = (B, T, self.engine_pref)
         p = self._programs.get(key)
         if p is None:
-            if self.engine is None:
-                self.engine = Engine()
-            if not self._uploaded:
-                self.engine.load_weights(self._blob)
-                self._uploaded = True
             pb = self.lower(B, T)
             p = Program(self.engine, pb)
             self._programs[key] = p
