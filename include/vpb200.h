@@ -363,6 +363,24 @@ size_t vp_gain_scratch_bytes(const vp_handle* h, int32_t B, int64_t ld);
 int vp_gain_normalize(vp_handle* h, float* wave, int64_t ld, int32_t B, const int64_t* lens, double target_db,
                       double max_gain_db, int32_t* flags, void* scratch, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Front of speaker_diarization (predict.py:365-379) on one device copy of the conditioned recording: the energy VAD's
+ * frame energies (mvector/audio.py, AudioSegment.vad) and the chunk rows (SpeakerDiarization._chunk).
+ * ---------------------------------------------------------------------------------------------------------- */
+/* out[f] (float64, device) <- (wave[:nf*hop].astype(float64).reshape(nf, hop) ** 2).mean(axis=1)[f] for f < nf = n / hop,
+ * bit-identical to numpy: each row is summed in numpy's pairwise order (below 8 elements sequentially from 0.0; up to 128
+ * with eight strided accumulators combined as ((r0+r1)+(r2+r3))+((r4+r5)+(r6+r7)), then the tail in order; above 128
+ * split at n2 = n/2 - (n/2) % 8 and the halves added) with __dadd_rn, then one __ddiv_rn by hop.  wave: n float32
+ * samples (device).  1 <= hop < 2^31; n < hop writes nothing.  NaN / inf propagate as in numpy.  Asynchronous on stream;
+ * no atomics. */
+int vp_frame_energy(vp_handle* h, const float* wave, int64_t n, int64_t hop, double* out, void* stream);
+/* dst[i, j] (float32 [n, ld], device) <- j < valid[i] ? src[offset[i] + j] : 0 for j < ld: window i of the device row
+ * src, zero filled past valid[i].  offset int64 [n], valid int32 [n], both device; src[offset[i] .. offset[i] +
+ * min(valid[i], ld)) must lie inside src (offsets past 2^31 elements are fine).  src and dst must not overlap.
+ * Asynchronous on stream. */
+int vp_gather_windows(vp_handle* h, const float* src, const int64_t* offset, const int32_t* valid, int64_t n, int64_t ld,
+                      float* dst, void* stream);
+
 /* Staging half of predict_batch (predict.py:244-255) as ONE native call: worker threads gather slices of slice_rows
  * utterances into the zero-padded PINNED matrix staging[n, lmax]; the calling thread -- one of the n_threads gatherers --
  * issues cudaMemcpyAsync(staging slice -> device_dst slice) on copy_stream, in slice order, as soon as a slice is

@@ -945,6 +945,28 @@ int vp_gain_normalize(vp_handle* h, float* wave, int64_t ld, int32_t B, const in
   return VP_OK;
 }
 
+int vp_frame_energy(vp_handle* h, const float* wave, int64_t n, int64_t hop, double* out, void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (n < 0 || hop < 1 || hop > INT32_MAX) return fail(h, VP_ERR_INVALID, "n = %lld, hop = %lld: need n >= 0, 1 <= hop < 2^31",
+                                                        (long long)n, (long long)hop);
+  if (n / hop == 0) return VP_OK;
+  if (!wave || !out) return fail(h, VP_ERR_INVALID, "null argument");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_frame_energy(wave, n / hop, hop, out, (cudaStream_t)stream));
+  return VP_OK;
+}
+
+int vp_gather_windows(vp_handle* h, const float* src, const int64_t* offset, const int32_t* valid, int64_t n, int64_t ld,
+                      float* dst, void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (n < 0 || ld < 0) return fail(h, VP_ERR_INVALID, "n = %lld, ld = %lld: negative", (long long)n, (long long)ld);
+  if (n == 0 || ld == 0) return VP_OK;
+  if (!src || !offset || !valid || !dst) return fail(h, VP_ERR_INVALID, "null argument");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_gather_windows(src, offset, valid, n, ld, dst, (cudaStream_t)stream));
+  return VP_OK;
+}
+
 int vp_program_peek(vp_program* p, int64_t off, size_t nbytes, void* dst, void* stream) {
   if (!p || !dst) return VP_ERR_INVALID;
   if (off < 0 || (size_t)off + nbytes > p->ws_bytes) return fail(p->h, VP_ERR_INVALID, "peek out of range");

@@ -91,6 +91,11 @@ size_t gain_scratch_bytes(int B, int64_t ld);
 cudaError_t launch_gain(float* w, int64_t ld, int B, const int64_t* lens, double target_db, double max_gain_db,
                         int32_t* flags, void* scratch, cudaStream_t stream);
 
+// diarization front: VAD frame energies and chunk windows of one device recording (segment.cu)
+cudaError_t launch_frame_energy(const float* x, int64_t nf, int64_t hop, double* out, cudaStream_t stream);
+cudaError_t launch_gather_windows(const float* src, const int64_t* offset, const int32_t* valid, int64_t rows, int64_t ld,
+                                  float* dst, cudaStream_t stream);
+
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);

@@ -121,6 +121,8 @@ def lib():
         'vp_gain_scratch_bytes': (sz, [vp, i32, C.c_int64]),
         'vp_gain_normalize': (C.c_int, [vp, f32p, C.c_int64, i32, C.c_void_p, C.c_double, C.c_double, C.c_void_p,
                                         C.c_void_p, vp]),
+        'vp_frame_energy': (C.c_int, [vp, f32p, C.c_int64, C.c_int64, C.c_void_p, vp]),
+        'vp_gather_windows': (C.c_int, [vp, f32p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, f32p, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = header/library mismatch
@@ -144,4 +146,4 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_frontend_plan_info', 'vp_cosine_scores', 'vp_device_zero',
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
            'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics',
-           'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize']
+           'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize', 'vp_frame_energy', 'vp_gather_windows']

@@ -104,6 +104,18 @@ class AudioSegment:
             raise ValueError(f'cannot normalise to {target_db} dB: gain {gain} dB exceeds {max_gain_db} dB')
         self.samples = (self.samples * (10.0 ** (gain / 20.0))).astype(np.float32)
 
+    @staticmethod
+    def vad_hop(sample_rate, frame_ms=30.0):
+        """Samples per VAD frame at ``sample_rate``."""
+        return max(1, int(sample_rate * frame_ms / 1000.0))
+
+    def frame_energy(self, frame_ms=30.0):
+        """Mean square of every whole VAD frame (float64 [n // hop]); ``Engine.frame_energy`` is its device twin."""
+        hop = self.vad_hop(self.sample_rate, frame_ms)
+        nf = self.samples.shape[0] // hop
+        x = self.samples[:nf * hop].astype(np.float64).reshape(nf, hop)
+        return (x * x).mean(axis=1)
+
     def vad(self, return_seconds=False, frame_ms=30.0, rel_threshold_db=-35.0, min_speech_ms=250.0, min_silence_ms=300.0):
         """Voice-activity segments ``[{'start': ..., 'end': ...}, ...]`` in samples (or seconds).
 
@@ -111,14 +123,18 @@ class AudioSegment:
         frame RMS energy against a threshold ``rel_threshold_db`` below the loudest frame, silences shorter than
         ``min_silence_ms`` bridged, bursts shorter than ``min_speech_ms`` dropped.  Same return format, so
         ``SpeakerDiarization.segments_audio`` (infer_utils/speaker_diarization.py) consumes either."""
-        sr = self.sample_rate
-        hop = max(1, int(sr * frame_ms / 1000.0))
-        n = self.samples.shape[0]
+        return self.vad_from_energy(self.frame_energy(frame_ms), self.samples.shape[0], self.sample_rate, return_seconds,
+                                    frame_ms, rel_threshold_db, min_speech_ms, min_silence_ms)
+
+    @classmethod
+    def vad_from_energy(cls, ms, n, sr, return_seconds=False, frame_ms=30.0, rel_threshold_db=-35.0, min_speech_ms=250.0,
+                        min_silence_ms=300.0):
+        """The decision half of ``vad``: ``ms`` the frame energies (``frame_energy``) of a recording of ``n`` samples at
+        ``sr`` Hz -> the same segments."""
+        hop = cls.vad_hop(sr, frame_ms)
         if n < hop:
             return []
-        nf = n // hop
-        x = self.samples[:nf * hop].astype(np.float64).reshape(nf, hop)
-        db = 10.0 * np.log10(np.maximum((x * x).mean(axis=1), 1e-12))
+        db = 10.0 * np.log10(np.maximum(np.asarray(ms, dtype=np.float64), 1e-12))
         active = db > (db.max() + rel_threshold_db)
         # runs of active frames
         edges = np.flatnonzero(np.diff(np.concatenate([[0], active.astype(np.int8), [0]])))

@@ -167,6 +167,26 @@ class Engine:
         plan.run(wave, wave.shape[1], y, y.shape[1], 0, B, flags, plan.scratch(B, y.shape[1]))
         return y, plan.n_out, flags
 
+    # ---- diarization front (csrc/segment.cu) ----
+    def frame_energy(self, wave, n, hop):
+        """VAD frame energies of the first ``n`` samples of the CUDA float32 row ``wave`` -> device float64 [n // hop],
+        bit-identical to AudioSegment.frame_energy (vp_frame_energy)."""
+        assert wave.is_cuda and wave.dtype == torch.float32 and wave.is_contiguous() and 0 <= n <= wave.numel()
+        out = torch.empty(n // hop, dtype=torch.float64, device=self.device)
+        _check(self._h, L.lib().vp_frame_energy(self._h, C.c_void_p(wave.data_ptr()), int(n), int(hop),
+                                                C.c_void_p(out.data_ptr()), self.stream_ptr()))
+        return out
+
+    def gather_windows(self, src, offset, valid, ld, dst, stream=None):
+        """Row i of ``dst`` [len(offset), ld] (CUDA float32, contiguous) <- ``src[offset[i]:offset[i] + valid[i]]``, zero
+        filled to ``ld`` samples (vp_gather_windows); ``offset`` / ``valid`` CUDA int64 / int32 vectors."""
+        n = offset.numel()
+        assert offset.dtype == torch.int64 and valid.dtype == torch.int32 and valid.numel() == n
+        assert src.is_cuda and src.dtype == torch.float32 and dst.dtype == torch.float32 and dst.numel() >= n * ld
+        sp = self.stream_ptr() if stream is None else C.c_void_p(stream.cuda_stream)
+        _check(self._h, L.lib().vp_gather_windows(self._h, C.c_void_p(src.data_ptr()), C.c_void_p(offset.data_ptr()),
+                                                  C.c_void_p(valid.data_ptr()), n, int(ld), C.c_void_p(dst.data_ptr()), sp))
+
     # ---- verification metrics (csrc/verify.cu) ----
     def verify(self, scores, labels=None, trial_labels=None, enroll_labels=None, p_target=0.01, c_miss=1, c_fa=1,
                sorted_out=False):

@@ -3,7 +3,8 @@ adapted from ModelScope).  The heavy step -- one embedding per 1.5 s chunk -- is
 sm_90a path; everything here is small host-side numpy / scipy / sklearn work on [n_chunks, embd] arrays, restated with
 the same interfaces, defaults and results as the reference classes:
 
-  SpeakerDiarization.segments_audio   VAD segments -> 1.5 s chunks every 0.75 s, last chunk right-aligned (:24-89)
+  SpeakerDiarization.segments_audio   VAD segments -> 1.5 s chunks every 0.75 s, last chunk right-aligned (:24-89);
+                                      chunk_table is the same cut as offsets into the recording, for a device copy
   SpeakerDiarization.clustering       spectral clustering -> relabel by first appearance -> speaker centres -> merge centres
                                       whose cosine exceeds merge_threshold (:91-135)
   SpeakerDiarization.postprocess      merge consecutive chunks of one speaker, split overlaps at the midpoint, absorb
@@ -15,6 +16,8 @@ the same interfaces, defaults and results as the reference classes:
 
 ``AudioSegment.vad`` (yeaudio's model-based VAD) is outside the parity boundary (SURVEY.md 8c); mvector.audio provides an
 energy-based stand-in with the same return format."""
+from typing import NamedTuple
+
 import numpy as np
 import scipy.linalg
 from sklearn.cluster import k_means
@@ -94,6 +97,16 @@ class SpectralCluster:
         return [b - a for a, b in zip(v[:-1], v[1:])]
 
 
+class ChunkTable(NamedTuple):
+    """The 1.5 s chunks of one recording (SpeakerDiarization.chunk_table): chunk i covers recording samples
+    offset[i] .. offset[i] + valid[i], zero filled to ``size`` samples, and the seconds start[i] .. end[i]."""
+    start: list
+    end: list
+    offset: np.ndarray
+    valid: np.ndarray
+    size: int
+
+
 class SpeakerDiarization(object):
     def __init__(self, seg_duration=1.5, seg_shift=0.75, sample_rate=16000, merge_threshold=0.78):
         self.seg_duration = seg_duration
@@ -111,31 +124,50 @@ class SpeakerDiarization(object):
     def segments_audio(self, audio_segment):
         """-> [[start s, end s, samples of one chunk], ...] over the voiced parts of the recording."""
         samples = audio_segment.samples
-        self.sample_rate = sr = audio_segment.sample_rate
-        voiced = []
-        for t in audio_segment.vad(return_seconds=True):
+        return self._slice(self.chunk_table(audio_segment.vad(return_seconds=True), samples.shape[0],
+                                            audio_segment.sample_rate), samples)
+
+    def chunk_table(self, vad_times, n, sr):
+        """The chunks of ``segments_audio`` without their samples: ``vad_times`` the VAD's segments in seconds over a
+        recording of ``n`` samples at ``sr`` Hz -> ChunkTable.  Raises the asserts ``segments_audio`` raises."""
+        self.sample_rate = sr
+        spans = []
+        for t in vad_times:
             st, ed = round(t['start'], 3), round(t['end'], 3)
-            voiced.append([st, ed, samples[int(st * sr):int(ed * sr)]])
-        self._check_audio_list(voiced)
-        return self._chunk(voiced)
+            r = range(n)[int(st * sr):int(ed * sr)]           # the samples slice samples[int(st sr):int(ed sr)] takes
+            spans.append((st, ed, r.start, len(r)))
+        self._check_spans([(st, ed, length) for st, ed, _, length in spans])
+        return self._chunk_table(spans)
 
     def _check_audio_list(self, audio):
+        """``audio``: [start s, end s, samples] per VAD segment."""
+        self._check_spans([(st, ed, data.shape[0] if isinstance(data, np.ndarray) else None) for st, ed, data in audio])
+
+    def _check_spans(self, spans):
+        """``spans``: (start s, end s, sample count or None for data that is not an array) per VAD segment."""
         total = 0
-        for i, (st, ed, data) in enumerate(audio):
+        for i, (st, ed, length) in enumerate(spans):
             assert ed >= st, '分割的时间戳错误'
-            assert isinstance(data, np.ndarray), '数据的类型不正确'
-            assert int(ed * self.sample_rate) - int(st * self.sample_rate) == data.shape[0], '时间长度和数据长度不匹配'
+            assert length is not None, '数据的类型不正确'
+            assert int(ed * self.sample_rate) - int(st * self.sample_rate) == length, '时间长度和数据长度不匹配'
             if i > 0:
-                assert st >= audio[i - 1][1], 'modelscope error: Wrong time stamps.'
+                assert st >= spans[i - 1][1], 'modelscope error: Wrong time stamps.'
             total += ed - st
         assert total > 5, f'音频时间过段，应当大于5秒，当前长度是{total}秒'
 
     def _chunk(self, vad_segments):
+        """``vad_segments``: [start s, end s, samples] per VAD segment -> [[start s, end s, chunk samples], ...]."""
+        out = []
+        for st, ed, data in vad_segments:
+            out += self._slice(self._chunk_table([(st, ed, 0, data.shape[0])]), data)
+        return out
+
+    def _chunk_table(self, spans):
+        """``spans``: (start s, end s, offset, sample count) per VAD segment -> ChunkTable of 1.5 s chunks every 0.75 s."""
         size = int(self.seg_duration * self.sample_rate)
         hop = int(self.seg_shift * self.sample_rate)
-        out = []
-        for seg_st, _, data in vad_segments:
-            n = data.shape[0]
+        start, end, offset, valid = [], [], [], []
+        for seg_st, _, base, n in spans:
             prev_end = 0
             for lo in range(0, n, hop):
                 hi = min(lo + size, n)
@@ -143,10 +175,22 @@ class SpeakerDiarization(object):
                     break
                 prev_end = hi
                 lo = max(0, hi - size)                         # the last chunk is right-aligned to the segment end
-                piece = data[lo:hi]
-                if piece.shape[0] < size:                      # segment shorter than one chunk: zero-pad
-                    piece = np.pad(piece, (0, size - piece.shape[0]), 'constant')
-                out.append([lo / self.sample_rate + seg_st, hi / self.sample_rate + seg_st, piece])
+                start.append(lo / self.sample_rate + seg_st)
+                end.append(hi / self.sample_rate + seg_st)
+                offset.append(base + lo)
+                valid.append(hi - lo)
+        return ChunkTable(start, end, np.array(offset, dtype=np.int64), np.array(valid, dtype=np.int32), size)
+
+    @staticmethod
+    def _slice(table, samples):
+        """ChunkTable over ``samples`` -> [[start s, end s, chunk samples], ...]; a chunk of a segment shorter than
+        ``size`` is zero padded."""
+        out = []
+        for st, ed, off, v in zip(table.start, table.end, table.offset.tolist(), table.valid.tolist()):
+            piece = samples[off:off + v]
+            if v < table.size:
+                piece = np.pad(piece, (0, table.size - v), 'constant')
+            out.append([st, ed, piece])
         return out
 
     # ------------------------------------------------------------------ clustering

@@ -8,10 +8,12 @@ Differences that are deliberate:
     the reference's ``batch_size`` argument (predict.py:261) is accepted and ignored -- chunking does not change
     results because every op is per-utterance, and padding/CMN/mask are computed on the full batch exactly like
     predict.py:244-258.
-  * ``speaker_diarization`` (predict.py:365-395): chunk embeddings come from ``predict_batch`` on the device, and
-    so does the spectral stage of the clustering up to its eigenvectors (``Engine.spectral_embedding``); chunking,
-    k-means and post-processing are host glue (infer_utils/speaker_diarization.py); the VAD is an energy
-    detector standing in for yeaudio's model-based one (absent third-party code, outside the parity boundary).
+  * ``speaker_diarization`` (predict.py:365-395): the recording is copied to the device once, at its native rate;
+    conditioning, the VAD's frame energies, the chunk rows, their embeddings and the spectral stage of the clustering up
+    to its eigenvectors (``Engine.spectral_embedding``) run there.  The VAD decision, the chunk table, k-means and
+    post-processing are host glue (audio.py, infer_utils/speaker_diarization.py) on per-frame and per-chunk numbers; the
+    VAD is an energy detector standing in for yeaudio's model-based one (absent third-party code, outside the parity
+    boundary).
 """
 import os
 import pickle
@@ -175,14 +177,16 @@ class MVectorPredictor:
             audio_segment = audio_data
         else:
             raise Exception(f'不支持该数据类型，当前数据类型为：{type(audio_data)}')
-        ds = self.configs.dataset_conf.dataset
-        assert audio_segment.duration >= ds.min_duration, \
-            f'音频太短，最小应该为{ds.min_duration}s，当前音频为{audio_segment.duration}s'
+        self._check_duration(audio_segment.duration)
         return audio_segment
 
+    def _check_duration(self, duration):
+        """predict.py:200-201: the too-short assert of one item of ``duration`` seconds at its native rate."""
+        ds = self.configs.dataset_conf.dataset
+        assert duration >= ds.min_duration, f'音频太短，最小应该为{ds.min_duration}s，当前音频为{duration}s'
+
     def _condition_host(self, audio_segment):
-        """predict.py:205-211 on the host, in place: ``register`` writes the normalised samples to disk and
-        ``speaker_diarization`` runs its VAD on them."""
+        """predict.py:205-211 on the host, in place: ``register`` writes the normalised samples to disk."""
         ds = self.configs.dataset_conf.dataset
         if audio_segment.sample_rate != ds.sample_rate:
             audio_segment.resample(ds.sample_rate)
@@ -297,8 +301,9 @@ class MVectorPredictor:
         return out
 
     def _embed_waves(self, waves, lmax, masked, to_numpy=True, group=None, rates=None):
-        """waves: list of 1-D float32 arrays, decoded, at ``rates`` Hz (None: all at the model's rate) -> [B, embd_dim]
-        (np.float32, or the device tensor with ``to_numpy=False``).  ``lmax`` is the longest item AFTER resampling.
+        """waves: list of 1-D float32 arrays, decoded, at ``rates`` Hz (None: all at the model's rate), or DeviceWindows
+        (rows already on the device) -> [B, embd_dim] (np.float32, or the device tensor with ``to_numpy=False``).
+        ``lmax`` is the longest item AFTER resampling.
 
         Conditioning (predict.py:205-211) runs on the device inside the staging: a stage with rows to resample is
         gathered at its native length into a native-rate device slot and resampled into the model-rate slot
@@ -315,7 +320,8 @@ class MVectorPredictor:
         slices finish (``vp_host_stage_h2d``) -- feed the fused front-end kernels, which run on the main stream behind an
         event of their stage's copies and write straight into the [B, T, F] feature buffer; as soon as the features of a
         backbone chunk (``_host_chunks``) are complete the main stream runs its program, under the next stage's gather and
-        copies.  One D2H of the result at the end."""
+        copies.  With DeviceWindows a stage's rows are written into its device slot by vp_gather_windows on the copy
+        stream instead; everything after that is the same.  One D2H of the result at the end."""
         from . import _lib as L
         import ctypes as C
         import time
@@ -337,7 +343,8 @@ class MVectorPredictor:
         lib = L.lib()
         F = fz.feature_dim
         ds_conf = self.configs.dataset_conf.dataset
-        lens = np.fromiter(map(len, waves), dtype=np.int32, count=B)
+        dev_rows = isinstance(waves, DeviceWindows)
+        lens = np.full(B, waves.size, dtype=np.int32) if dev_rows else np.fromiter(map(len, waves), dtype=np.int32, count=B)
         plan = None
         gain_db = ds_conf.target_dB if ds_conf.use_dB_normalization else None
         if gain_db is not None or (rates is not None and any(int(r) != ds_conf.sample_rate for r in rates)):
@@ -390,24 +397,30 @@ class MVectorPredictor:
             g1 = min(g0 + S, B)
             n = g1 - g0
             ps, ds = gi & 1, gi % K
-            if pin_ev[ps] is not None:
-                pin_ev[ps].synchronize()
             if dev_ev[ds] is not None:
                 cs.wait_event(dev_ev[ds])
             dw = dwave[ds]
             resample = plan is not None and plan.rows_resampled(g0, g1)
             ld = int(lens[g0:g1].max()) if resample else lmax          # a resampling stage stages its native rows
             dst = dnat[ds] if resample else dw
-            host = self._pinned_slot(ps, n * ld)
-            ptrs[g0:g1] = np.fromiter((w.__array_interface__['data'][0] for w in waves[g0:g1]), dtype=np.uint64, count=n)
-            rc = lib.vp_host_stage_h2d(C.c_void_p(ptrs.ctypes.data + 8 * g0), C.c_void_p(lens.ctypes.data + 4 * g0), n, ld,
-                                       C.c_void_p(host.data_ptr()), C.c_void_p(dst.data_ptr()), self.COPY_SLICE, nthreads, cs_ptr)
-            if rc != L.VP_OK:
-                raise L.VpError(rc, 'vp_host_stage_h2d failed')
-            mark(f'stage {gi}: {n} utterances gathered, H2D enqueued')
+            if dev_rows:
+                waves.gather(g0, g1, dst, ld, cs)
+                mark(f'stage {gi}: {n} windows gathered on the device')
+            else:
+                if pin_ev[ps] is not None:
+                    pin_ev[ps].synchronize()
+                host = self._pinned_slot(ps, n * ld)
+                ptrs[g0:g1] = np.fromiter((w.__array_interface__['data'][0] for w in waves[g0:g1]), dtype=np.uint64, count=n)
+                rc = lib.vp_host_stage_h2d(C.c_void_p(ptrs.ctypes.data + 8 * g0), C.c_void_p(lens.ctypes.data + 4 * g0), n,
+                                           ld, C.c_void_p(host.data_ptr()), C.c_void_p(dst.data_ptr()), self.COPY_SLICE,
+                                           nthreads, cs_ptr)
+                if rc != L.VP_OK:
+                    raise L.VpError(rc, 'vp_host_stage_h2d failed')
+                mark(f'stage {gi}: {n} utterances gathered, H2D enqueued')
             cev = torch.cuda.Event()
             cev.record(cs)
-            pin_ev[ps] = cev
+            if not dev_rows:
+                pin_ev[ps] = cev
             dmark(f'stage {gi}: H2D done', cs)
             main.wait_event(cev)
             if plan is not None:
@@ -563,17 +576,63 @@ class MVectorPredictor:
         return True
 
     def speaker_diarization(self, audio_data, sample_rate=16000, speaker_num=None, search_audio_db=False):
-        """说话人日志识别 (predict.py:365-395) -> [{'speaker': id or name, 'start': s, 'end': s}, ...]"""
-        input_data = self._condition_host(self._load_audio(audio_data=audio_data, sample_rate=sample_rate))
-        # the 16 kHz chunks go to predict_batch with the caller's sample_rate, as in the reference (predict.py:379): a
-        # caller at another rate has them resampled a second time
-        segments = self.speaker_diarize.segments_audio(input_data)
-        features = self.predict_batch([seg[2] for seg in segments], sample_rate=sample_rate)
+        """说话人日志识别 (predict.py:365-395) -> [{'speaker': id or name, 'start': s, 'end': s}, ...]
+
+        The decoded recording is copied to the device once, at its native rate, and conditioned there
+        (``Engine.condition``); its VAD frame energies are computed there too (``Engine.frame_energy``), so only those
+        numbers come back for the VAD decision and the chunk table (``SpeakerDiarization.chunk_table``).  The chunk rows
+        are cut from the device recording by the staging of ``_embed_waves`` (DeviceWindows), which then embeds them as
+        ``predict_batch`` embeds host chunks: same conditioning plan, front-end and backbone split, so the embeddings
+        are the same bits."""
+        seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
+        ds = self.configs.dataset_conf.dataset
+        eng = self._engine
+        x = torch.from_numpy(np.ascontiguousarray(seg.samples, dtype=np.float32)).to(self.device)
+        gain_db = ds.target_dB if ds.use_dB_normalization else None
+        y, n_out, flags = eng.condition(x.view(1, -1), [x.numel()], [seg.sample_rate], ds.sample_rate, gain_db)
+        n, sr = int(n_out[0]), int(ds.sample_rate)
+        y = y.view(-1)
+        energy = eng.frame_energy(y, n, AudioSegment.vad_hop(sr)).cpu().numpy()
+        if flags is not None and flags.cpu().numpy().any():  # a silent recording: _condition_host's ValueError
+            eng.condition_plan([x.numel()], [seg.sample_rate], sr, gain_db).check(flags.cpu().numpy(), [seg.samples])
+        table = self.speaker_diarize.chunk_table(AudioSegment.vad_from_energy(energy, n, sr, return_seconds=True), n, sr)
+        # the chunks go on with the caller's sample_rate, as in the reference (predict.py:379): a caller at another rate
+        # has them resampled a second time, and predict_batch's too-short assert applies to each of them
+        rate = int(sample_rate)
+        self._check_duration(table.size / float(rate))
+        lmax = int(self._output_lengths([table.size], [rate])[0])
+        features = self._embed_waves(DeviceWindows(eng, y, table), lmax, masked=True, rates=[rate] * len(table.start))
         labels, spk_center_embeddings = self.speaker_diarize.clustering(features, speaker_num=speaker_num)
-        outputs = self.speaker_diarize.postprocess(segments, labels)
+        outputs = self.speaker_diarize.postprocess([[st, ed] for st, ed in zip(table.start, table.end)], labels)
         if search_audio_db:
             assert self.audio_feature is not None, "数据库中没有音频数据，请先指定说话人特征数据库或者注册说话人"
             names = self.__retrieval(np_feature=spk_center_embeddings)
             outputs = [{'speaker': names[o['speaker']][0] if names[o['speaker']][0] else f"陌生人{o['speaker']}",
                         'start': o['start'], 'end': o['end']} for o in outputs]
         return outputs
+
+
+class DeviceWindows:
+    """Rows of ``_embed_waves`` cut from one device recording ``src`` by a ChunkTable: row i is
+    src[offset[i]:offset[i] + valid[i]] zero filled to ``size`` samples.  A staging slot is written by vp_gather_windows
+    instead of the host gather and H2D copy."""
+
+    def __init__(self, engine, src, table):
+        self.engine, self.src, self.table = engine, src, table
+        self.size = int(table.size)
+        self._offset = torch.from_numpy(table.offset).to(src.device)
+        self._valid = torch.from_numpy(table.valid).to(src.device)
+
+    def __len__(self):
+        return len(self.table.start)
+
+    def __getitem__(self, i):
+        """Host copy of row i (ConditionPlan.check recomputes a flagged row's gain from it)."""
+        o, v = int(self.table.offset[i]), int(self.table.valid[i])
+        row = np.zeros(self.size, dtype=np.float32)
+        row[:v] = self.src[o:o + v].cpu().numpy()
+        return row
+
+    def gather(self, lo, hi, dst, ld, stream):
+        """Rows lo..hi into the device slot ``dst`` [hi - lo, ld] on ``stream``."""
+        self.engine.gather_windows(self.src, self._offset[lo:hi], self._valid[lo:hi], ld, dst, stream)
