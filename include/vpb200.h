@@ -219,8 +219,10 @@ typedef struct vp_op {
    * every vp_embed) behind the program workspace.  An op with amax_out = s + 1 atomically maxes |y| over everything it
    * writes into slot s (max is exact and order independent: results stay deterministic); a CONV with amax_in = s + 1 may
    * run on the fp16 split and then scales its gathered activations by the power of two that puts slot s's maximum just
-   * below 2^14, so the split is range-safe whatever the magnitude of the activations.  0 = none: the op then never runs
-   * on the fp16 split (it stays on split-TF32, which has fp32's range). */
+   * below 2^14, so the split keeps its accuracy for a slot maximum anywhere from 2^-113 up to the largest finite float.
+   * (Below 2^-113 the scale would leave fp32's normal range; such a tensor's products lie among fp32's subnormals,
+   * where the fp32 reference itself has lost bits.)  0 = none: the op then never runs on the fp16 split (it stays on
+   * split-TF32, which has fp32's range). */
   int32_t amax_out, amax_in;
   /* Accumulation chunk of the tensor-core engines: 0 = the whole K extent goes into one accumulator; > 0 (a multiple of
    * 64) = every tc_kc K elements go into a fresh accumulator and the consumer warps fold the chunks with correctly

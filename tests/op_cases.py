@@ -910,17 +910,27 @@ AMAX_WRITERS = dict(
 AMAX_KERNELS = dict(ew_gate_res='ew', ew_aff='ew', pad_copy='pad_copy', pool2d='pool2d', c1_wide='conv_c1_wide',
                     c1_generic='conv_c1', ffma_conv='conv_ffma<64>', tf32_conv='conv_tc<tf32>',
                     tc16_conv='conv_tc<f16>', tc16_wide_conv='conv_tc16_wide', small_m_1024='linear_small_m')
-RANGE_SCALES = (1e-30, 1e-6, 1e6, 1e30)
+# 2^-110 and 2^116 lie past the +-100 clamp the fp16 split's scale exponent once had (its lo terms fell to fp16
+# subnormals below max|x| = 2^-87, its hi terms overflowed from 2^116); every writer's output stays in fp32's normal range
+RANGE_SCALES = (2.0 ** -110, 1e-30, 1e-6, 1e6, 1e30, 2.0 ** 116)
+
+
+def scale_name(s):
+    """'1e-30' for the decimal scales, '2^-110' for the powers of two."""
+    e = np.log2(s)
+    return f'2^{int(e)}' if e == int(e) and abs(e) > 100 else f'{s:g}'
+
+
 # the scale multiplies every input AND the writers' biases, so the tensor the consumer reads is O(scale) at both ends
 # of the sweep (an unscaled bias of ~0.1 would run the small-scale half at unit scale)
 AMAX_CASES = {}
 for _i, (_name, _w) in enumerate(AMAX_WRITERS.items()):
     for _s in RANGE_SCALES:
-        AMAX_CASES[f'{_name}-{_s:g}'] = dict(_w, seed=400 + _i, scale=_s, bias_scale=_s, kernel=AMAX_KERNELS[_name],
+        AMAX_CASES[f'{_name}-{scale_name(_s)}'] = dict(_w, seed=400 + _i, scale=_s, bias_scale=_s, kernel=AMAX_KERNELS[_name],
                                              consumer=_CONSUMER)
 # linear_small_m at M = 1024: the only M that is both small-M (FFMA) and tensor-core eligible for its consumer
 for _s in RANGE_SCALES:
-    AMAX_CASES[f'small_m_1024-{_s:g}'] = dict(op='conv', engine='ffma', B=4, Tin=256, Cin=64, N=64, bias=True, out_C=64,
+    AMAX_CASES[f'small_m_1024-{scale_name(_s)}'] = dict(op='conv', engine='ffma', B=4, Tin=256, Cin=64, N=64, bias=True, out_C=64,
                                               seed=420, scale=_s, bias_scale=_s, kernel='linear_small_m',
                                               consumer=dict(B=4, T=256, N=128))
 # two writers into column windows of ONE allocation at scales 1e6 (FFMA conv) and 1 (EW residual add), one consumer
@@ -935,11 +945,11 @@ SHARED_SLOT_CASES = {
 # slot reset between graph replays: EW copy -> TC16 conv, run at 1e30, then at 1e-30 through the captured graph
 GRAPH_RESET = dict(op='ew', mode='COPY', B=4, T=300, C=64, out_C=64, seed=440, kernel='ew', consumer=_CONSUMER)
 
-# one 512 x 512 GEMM over 8 x 298 rows (EW copy -> TC16 conv) at input scales 1e-30 ... 1e30: the fp16 split neither
+# one 512 x 512 GEMM over 8 x 298 rows (EW copy -> TC16 conv) at input scales 2^-110 ... 2^116: the fp16 split neither
 # overflows (|x| > 65504) nor loses small tensors to fp16 subnormals, its error does not depend on the magnitude
-TC16_RANGE_CASES = {f'gemm_512-{_s:g}': dict(op='ew', mode='COPY', B=8, T=298, C=512, out_C=512, seed=450, scale=_s,
-                                             kernel='ew', consumer=dict(B=8, T=298, N=512))
-                    for _s in (1e-30, 1e-8, 1e-3, 1e4, 1e9, 1e30)}
+TC16_RANGE_CASES = {f'gemm_512-{scale_name(_s)}': dict(op='ew', mode='COPY', B=8, T=298, C=512, out_C=512, seed=450,
+                                                       scale=_s, kernel='ew', consumer=dict(B=8, T=298, N=512))
+                    for _s in (2.0 ** -110, 1e-30, 1e-8, 1e-3, 1e4, 1e9, 1e30, 2.0 ** 116)}
 
 # ---- the fp16 split's wide path (conv_tc16_wide_kernel, tests/test_gpu_tc16_wide.py): 128 x 256 tiles for pointwise,
 # stride-1, unpadded, unchunked convs with one plain source and N % 256 == 0, N >= 1024 (tc16_wide_ok).  Its edges, and
@@ -964,6 +974,8 @@ _wide('tiles_152', 209, B=8, Tin=300, Cin=128, N=2048, bias=True, act=L.ACT_RELU
 _wide('general_epilogue', 210, B=4, Tin=300, Cin=128, N=1024, bias=True, ubias=True, act=L.ACT_SILU)
 _wide('scale_1e-30', 211, B=4, Tin=300, Cin=512, N=1024, bias=True, bias_scale=1e-30, scale=1e-30)
 _wide('scale_1e+30', 212, B=4, Tin=300, Cin=512, N=1024, bias=True, bias_scale=1e30, scale=1e30)
+_wide('scale_2^-110', 223, B=4, Tin=300, Cin=512, N=1024, bias=True, bias_scale=2.0 ** -110, scale=2.0 ** -110)
+_wide('scale_2^116', 224, B=4, Tin=300, Cin=512, N=1024, bias=True, bias_scale=2.0 ** 116, scale=2.0 ** 116)
 # several tiles per CTA with an odd K-block count: the 2-stage ring's stage index and phase carry over from one tile to
 # the next on the other parity, and the next tile's residual is prefetched; 63 x 4 tiles with a 64-row M tail
 _wide('multi_tile_odd_k', 213, B=8, Tin=1000, Cin=192, N=1024, bias=True, act=L.ACT_RELU, res=True,

@@ -121,14 +121,28 @@ __device__ __forceinline__ void amax_commit_block(unsigned* slot, float m) {
   }
 }
 
-// exponent s such that amax * 2^s lies in [2^13, 2^14): fp16 hi terms stay below 65504, lo terms above the subnormals
+// exponent s such that amax * 2^s lies in [2^13, 2^14): fp16 hi terms stay below 65504, lo terms above the subnormals.
+// That holds for every amax from 2^-113 up to the largest finite float (s from 126 down to -114, both normal powers of
+// two for exp2i).  Below 2^-113 s stays at 126 and the lo terms of the scaled tensor reach fp16's subnormals; such a
+// tensor's products are themselves down among fp32's subnormals, where the fp32 reference has lost as many bits.
 __device__ __forceinline__ int f16_scale_exp(unsigned amax_bits) {
   const int be = (int)((amax_bits >> 23) & 0xffu);
   if (amax_bits == 0u || be == 0xff) return 0;          // all-zero tensor, or inf / nan (propagates like the reference)
-  int s = 13 - (be - 127);
-  return s < -100 ? -100 : (s > 100 ? 100 : s);
+  const int s = 13 - (be - 127);
+  return s > 126 ? 126 : s;                             // be >= 0: s >= -114
 }
 __device__ __forceinline__ float exp2i(int s) { return __uint_as_float((unsigned)(s + 127) << 23); }
+
+// The fp16 split's descale 2^-k (weight image, a normal power of two) x 2^-s (activation scale), its exponents combined
+// as integers: the float product of the two factors would overflow past 2^127 (large weights, k < 0) or lose the
+// subnormal range.  2^(-k-s) is exact down to 2^-149, a subnormal power of two, and the epilogue's fma still rounds the
+// descaled accumulator once.  Below 2^-149 every product |x w| is below 2^-121 (both scaled maxima are below 2^14), so
+// the descale is 0: such outputs lie at fp32's subnormal edge.  Above 2^127 the largest product already exceeds fp32.
+__device__ __forceinline__ float f16_descale(float w_descale, int s) {
+  const int e = (int)((__float_as_uint(w_descale) >> 23) & 0xffu) - 127 - s;
+  if (e >= -126) return exp2i(e < 127 ? e : 127);
+  return e < -149 ? 0.f : __uint_as_float(1u << (e + 149));
+}
 
 // Decoded A-operand row (one output position): where its receptive field starts in the source map.
 struct RowInfo {

@@ -133,7 +133,8 @@ __device__ __noinline__ float2 act2_slow(float2 v, int act) {
 struct Epi {
   bool simple, relu, relu2, need_urow;
   float hi1, hi2;
-  float descale;         // fp16 split: 2^-k of the weight image x 2^-s of the activation scale; 1 on the tf32 path
+  float descale;         // fp16 split: 2^-k of the weight image x 2^-s of the activation scale (f16_descale); 1 on the
+                         // tf32 path
 };
 __device__ __forceinline__ Epi make_epi(const ConvParams& p, float descale) {
   auto clamps = [](int act) { return act == VP_ACT_RELU || act == VP_ACT_HARDTANH20; };
@@ -401,7 +402,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
       int p_s = 0;
       uint32_t p_ph = 0;
       // fp16 split: dynamic power-of-two activation scale from the source tensor's amax slot (written by the ops that
-      // produced the tensor, complete at kernel start) -> |x * ascale| < 2^14, range-safe for any activation magnitude
+      // produced the tensor, complete at kernel start) -> |x * ascale| < 2^14 for max|x| >= 2^-113 (f16_scale_exp)
       float ascale = 1.f;
       if constexpr (F16) ascale = exp2i(f16_scale_exp(__ldg(p.amax_in)));
       auto publish = [&](int q, SlotT& sl) {
@@ -492,7 +493,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) conv_tc_kernel(const __grid_co
     int s = 0;
     uint32_t sph = 0;                                         // stage / phase cursors, advanced without divisions
     float descale = 1.f;                                      // fp16 split: 2^-k of the weight image x 2^-s of the activation scale
-    if constexpr (F16) descale = a.descale * exp2i(-f16_scale_exp(__ldg(p.amax_in)));
+    if constexpr (F16) descale = f16_descale(a.descale, f16_scale_exp(__ldg(p.amax_in)));
     float tmax = 0.f;                                         // running max |y| of everything this thread stores (amax_out slot)
     const Epi epi = make_epi(p, descale);
     for (int g = blockIdx.x; g < total_groups; g += gridDim.x) {
@@ -715,7 +716,7 @@ __global__ void __launch_bounds__(W_THREADS, 1) conv_tc16_wide_kernel(const __gr
   const int rbase = 64 * wg + 16 * (warp & 3) + (lane >> 2);   // fragment rows rbase and rbase + 8 of the tile
   const int sexp = f16_scale_exp(__ldg(p.amax_in));
   const float ascale = exp2i(sexp);
-  const Epi epi = make_epi(p, a.descale * exp2i(-sexp));
+  const Epi epi = make_epi(p, f16_descale(a.descale, sexp));
   float acc[WBN / 2];
 #pragma unroll
   for (int i = 0; i < WBN / 2; ++i) acc[i] = 0.f;
