@@ -383,6 +383,43 @@ int vp_frame_energy(vp_handle* h, const float* wave, int64_t n, int64_t hop, dou
 int vp_gather_windows(vp_handle* h, const float* src, const int64_t* offset, const int32_t* valid, int64_t n, int64_t ld,
                       float* dst, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * FLAC decoding (RFC 9639) of B native streams on the device, 4-24 bits per sample, 1-8 channels, every frame and
+ * subframe coding the RFC defines for those depths.  CRC-8 is checked on every frame header and CRC-16 on every frame;
+ * the STREAMINFO MD5 of the audio is not checked.
+ * ---------------------------------------------------------------------------------------------------------- */
+typedef struct vp_flac_info {  /* a stream's STREAMINFO (mvector/flac.py parses it on the host) */
+  int64_t total_samples;       /* samples per channel, >= 1 (0 = unknown is not accepted) */
+  int32_t sample_rate;
+  int32_t channels;            /* 1..8 */
+  int32_t bps;                 /* bits per sample, 4..24 */
+  int32_t min_blocksize;       /* >= 16 */
+  int32_t max_blocksize;       /* min_blocksize..65535 */
+  int32_t min_framesize;       /* bytes, 0 = unknown */
+  int32_t max_framesize;       /* bytes, 0 = unknown */
+  int32_t reserved0;
+} vp_flac_info;
+int32_t vp_sizeof_flac_info(void);   /* binding self-check: sizeof(vp_flac_info) */
+/* Device scratch bytes of one vp_flac_decode: about 5 bytes per input byte plus 8 per frame slot.  max_frames: the frame
+ * slots of the batch, at least the sum over its streams of ceil(total_samples / min_blocksize). */
+size_t vp_flac_scratch_bytes(const vp_handle* h, int32_t B, int64_t nbytes, int64_t max_frames);
+/* data: the nbytes concatenated bytes of the B streams (device); the scan pass and the scratch cover exactly nbytes, so a
+ * batch whose stream_off is not ordered inside [0, nbytes] has every stream refused (status 1) before any stream byte is
+ * read.  stream_off int64 [B + 1]: stream b is data[stream_off[b] .. stream_off[b + 1]); frame_off int64 [B]: absolute offset of its first frame (the byte after its
+ * last metadata block); info [B]: its STREAMINFO.  All device.
+ * out [B, ld] float32 (device): row b <- the stream decoded, the channels of each sample mixed exactly as
+ * mvector.audio.pcm_to_mono mixes the same integers (x / 2^(bps-1) in float32, then numpy's float32 mean over the
+ * channels: left to right below 8 channels, ((c0+c1)+(c2+c3))+((c4+c5)+(c6+c7)) for 8, one division by the count; the
+ * stereo decorrelations first), zero filled from total_samples to ld.
+ * status int32 [B] (device) <- 0, or a non-zero OR of reasons: 1 STREAMINFO out of range (or total_samples > ld, or the
+ * frame table would pass max_frames, or stream_off out of order or past nbytes), 2 no frame proven at frame_off, 4 frames that do not tile [0, total_samples)
+ * exactly, 8 a frame header contradicting STREAMINFO, 16 a subframe with a reserved code, an out-of-range value or a
+ * decode that does not end at the frame's CRC-16.  A refused row's samples are unspecified; the other rows are exact.
+ * Every read of a stream stays inside its own byte range.  Asynchronous on stream. */
+int vp_flac_decode(vp_handle* h, const uint8_t* data, const int64_t* stream_off, const int64_t* frame_off,
+                   const vp_flac_info* info, int32_t B, float* out, int64_t ld, int32_t* status, void* scratch,
+                   int64_t nbytes, int64_t max_frames, void* stream);
+
 /* Staging half of predict_batch (predict.py:244-255) as ONE native call: worker threads gather slices of slice_rows
  * utterances into the zero-padded PINNED matrix staging[n, lmax]; the calling thread -- one of the n_threads gatherers --
  * issues cudaMemcpyAsync(staging slice -> device_dst slice) on copy_stream, in slice order, as soon as a slice is

@@ -967,6 +967,30 @@ int vp_gather_windows(vp_handle* h, const float* src, const int64_t* offset, con
   return VP_OK;
 }
 
+int32_t vp_sizeof_flac_info(void) { return (int32_t)sizeof(vp_flac_info); }
+
+size_t vp_flac_scratch_bytes(const vp_handle* h, int32_t B, int64_t nbytes, int64_t max_frames) {
+  (void)h;
+  return B < 1 || nbytes < 0 || max_frames < 0 ? 0 : flac_scratch_bytes(B, nbytes, max_frames);
+}
+
+int vp_flac_decode(vp_handle* h, const uint8_t* data, const int64_t* stream_off, const int64_t* frame_off,
+                   const vp_flac_info* info, int32_t B, float* out, int64_t ld, int32_t* status, void* scratch,
+                   int64_t nbytes, int64_t max_frames, void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (B < 0 || B > 65535) return fail(h, VP_ERR_UNSUPPORTED, "B = %d outside [0, 65535]", B);
+  if (B == 0) return VP_OK;
+  if (nbytes < 0 || max_frames < 0 || ld < 0)
+    return fail(h, VP_ERR_INVALID, "nbytes = %lld, max_frames = %lld, ld = %lld: negative", (long long)nbytes,
+                (long long)max_frames, (long long)ld);
+  if ((nbytes && !data) || !stream_off || !frame_off || !info || !out || !status || !scratch)
+    return fail(h, VP_ERR_INVALID, "null argument");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_flac_decode(data, nbytes, stream_off, frame_off, info, B, max_frames, out, ld, status, scratch,
+                                 (cudaStream_t)stream));
+  return VP_OK;
+}
+
 int vp_program_peek(vp_program* p, int64_t off, size_t nbytes, void* dst, void* stream) {
   if (!p || !dst) return VP_ERR_INVALID;
   if (off < 0 || (size_t)off + nbytes > p->ws_bytes) return fail(p->h, VP_ERR_INVALID, "peek out of range");

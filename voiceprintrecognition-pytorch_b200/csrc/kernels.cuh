@@ -96,6 +96,12 @@ cudaError_t launch_frame_energy(const float* x, int64_t nf, int64_t hop, double*
 cudaError_t launch_gather_windows(const float* src, const int64_t* offset, const int32_t* valid, int64_t rows, int64_t ld,
                                   float* dst, cudaStream_t stream);
 
+// FLAC decoding: scan, link and decode passes over B concatenated streams (flac.cu)
+size_t flac_scratch_bytes(int B, int64_t nbytes, int64_t max_frames);
+cudaError_t launch_flac_decode(const uint8_t* data, int64_t nbytes, const int64_t* stream_off, const int64_t* frame_off,
+                               const vp_flac_info* info, int B, int64_t max_frames, float* out, int64_t ld,
+                               int32_t* status, void* scratch, cudaStream_t stream);
+
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);

@@ -54,6 +54,12 @@ class VerifyResult(C.Structure):
                 + [('min_cost', C.c_double), ('argmin', C.c_int64), ('threshold', C.c_float), ('reserved0', C.c_int32)])
 
 
+class FlacInfo(C.Structure):
+    _fields_ = [('total_samples', C.c_int64), ('sample_rate', C.c_int32), ('channels', C.c_int32), ('bps', C.c_int32),
+                ('min_blocksize', C.c_int32), ('max_blocksize', C.c_int32), ('min_framesize', C.c_int32),
+                ('max_framesize', C.c_int32), ('reserved0', C.c_int32)]
+
+
 class VpError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f'vpb200 error {code}: {msg}')
@@ -123,6 +129,10 @@ def lib():
                                         C.c_void_p, vp]),
         'vp_frame_energy': (C.c_int, [vp, f32p, C.c_int64, C.c_int64, C.c_void_p, vp]),
         'vp_gather_windows': (C.c_int, [vp, f32p, C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, f32p, vp]),
+        'vp_sizeof_flac_info': (i32, []),
+        'vp_flac_scratch_bytes': (sz, [vp, i32, C.c_int64, C.c_int64]),
+        'vp_flac_decode': (C.c_int, [vp, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, i32, f32p, C.c_int64,
+                                     C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = header/library mismatch
@@ -131,8 +141,8 @@ def lib():
     if L.vp_abi_version() != 4:
         raise RuntimeError('libvpb200.so ABI version mismatch')
     if L.vp_sizeof_op() != C.sizeof(Op) or L.vp_sizeof_frontend_desc() != C.sizeof(FrontendDesc) \
-            or L.vp_sizeof_frontend_options() != C.sizeof(FrontendOptions):
-        raise RuntimeError('vp_op / vp_frontend_desc / vp_frontend_options layout mismatch between the ctypes binding '
+            or L.vp_sizeof_frontend_options() != C.sizeof(FrontendOptions) or L.vp_sizeof_flac_info() != C.sizeof(FlacInfo):
+        raise RuntimeError('vp_op / vp_frontend_desc / vp_frontend_options / vp_flac_info layout mismatch between the ctypes binding '
                            'and libvpb200.so')
     _lib = L
     return L
@@ -146,4 +156,5 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_frontend_plan_info', 'vp_cosine_scores', 'vp_device_zero',
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
            'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics',
-           'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize', 'vp_frame_energy', 'vp_gather_windows']
+           'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize', 'vp_frame_energy', 'vp_gather_windows',
+           'vp_sizeof_flac_info', 'vp_flac_scratch_bytes', 'vp_flac_decode']

@@ -2,8 +2,11 @@
 ``samples`` (float32 mono in [-1, 1]), ``sample_rate``, ``duration``, ``from_file`` / ``from_ndarray`` / ``from_bytes``,
 ``resample``, ``normalize``, ``vad``.  yeaudio (requirements.txt:12) is a third-party package absent from the reference tree and
 from this image; decoding/resampling sit OUTSIDE the parity boundary (SURVEY.md 8a3: parity starts at identical
-waveforms).  Decoding covers PCM WAV via the standard library only."""
+waveforms).  Decoding covers PCM WAV via the standard library and native FLAC (RFC 9639) on the device: a FLAC segment
+knows its rate and duration from STREAMINFO and is decoded by vp_flac_decode the first time its samples are read.  Both
+formats turn their integers into float32 mono with ``pcm_to_mono``."""
 import io
+import os
 import wave
 from math import gcd
 
@@ -41,6 +44,50 @@ def polyphase_taps(up, down):
     return np.ascontiguousarray(flat.reshape(nt, up).T).reshape(-1), nt, (half_len + n_pre_pad) // down
 
 
+def pcm_to_mono(ints, channels, bps):
+    """Interleaved integer PCM -> float32 mono: x / 2^(bps - 1) in float32, then (channels > 1) numpy's float32 mean over
+    each sample's channels.  vp_flac_decode reproduces this bit for bit (include/vpb200.h)."""
+    x = np.asarray(ints).astype(np.float32) / np.float32(2 ** (bps - 1))
+    if channels > 1:
+        x = x.reshape(-1, channels).mean(axis=1)
+    return x
+
+
+_engines = {}
+
+
+def _engine(device=None):
+    """The Engine FLAC segments decode with: one per CUDA device (default: the current one)."""
+    import torch
+    from .engine import Engine
+    idx = torch.cuda.current_device() if device is None else torch.device(device).index
+    if idx not in _engines:
+        _engines[idx] = Engine(idx)
+    return _engines[idx]
+
+
+def device_samples(seg, engine):
+    """A segment's samples as a CUDA float32 row on ``engine``'s device: an undecoded FLAC segment is decoded there and
+    its PCM never visits the host; any other segment's samples are uploaded."""
+    import torch
+    if isinstance(seg, FlacSegment) and seg._samples is None:
+        return seg.decode_device(engine)
+    return torch.from_numpy(np.ascontiguousarray(seg.samples, dtype=np.float32)).to(engine.device)
+
+
+def decode_segments(segs, engine=None):
+    """Give every undecoded FlacSegment of ``segs`` its host samples with ONE device decode (ValueError names a
+    refused item)."""
+    todo = [s for s in segs if isinstance(s, FlacSegment) and s._samples is None]
+    if not todo:
+        return
+    eng = engine or _engine()
+    rows, _ = eng.decode_flac([s.data for s in todo], [s.info for s in todo], [s.name for s in todo])
+    host = rows.cpu().numpy()
+    for s, r in zip(todo, host):
+        s._samples = np.ascontiguousarray(r[:s.info.total_samples])
+
+
 class AudioSegment:
     def __init__(self, samples, sample_rate):
         s = np.asarray(samples)
@@ -66,23 +113,35 @@ class AudioSegment:
             n, ch, sw, sr = w.getnframes(), w.getnchannels(), w.getsampwidth(), w.getframerate()
             raw = w.readframes(n)
         if sw == 2:
-            pcm = np.frombuffer(raw, dtype='<i2').astype(np.float32) / 32768.0
+            ints = np.frombuffer(raw, dtype='<i2')
         elif sw == 4:
-            pcm = np.frombuffer(raw, dtype='<i4').astype(np.float32) / 2147483648.0
+            ints = np.frombuffer(raw, dtype='<i4')
         elif sw == 1:
-            pcm = (np.frombuffer(raw, dtype=np.uint8).astype(np.float32) - 128.0) / 128.0
+            ints = np.frombuffer(raw, dtype=np.uint8).astype(np.int16) - 128
         else:
             raise ValueError(f'unsupported WAV sample width {sw}')
-        if ch > 1:
-            pcm = pcm.reshape(-1, ch).mean(axis=1)
-        return cls(pcm, sr)
+        return cls(pcm_to_mono(ints, ch, 8 * sw), sr)
 
     @classmethod
     def from_file(cls, file):
-        return cls._from_wave(file)
+        """A WAV or native FLAC file (path or binary file object), told apart by the FLAC magic."""
+        from .flac import is_flac
+        if isinstance(file, (str, os.PathLike)):
+            with open(file, 'rb') as f:
+                if not is_flac(f.read(4)):
+                    return cls._from_wave(file)
+                f.seek(0)
+                return FlacSegment(f.read(), name=os.fspath(file))
+        data = file.read()
+        if is_flac(data):
+            return FlacSegment(data, name=getattr(file, 'name', '<file>'))
+        return cls._from_wave(io.BytesIO(data))
 
     @classmethod
     def from_bytes(cls, data):
+        from .flac import is_flac
+        if is_flac(data):
+            return FlacSegment(data, name='<bytes>')
         return cls._from_wave(io.BytesIO(data))
 
     def resample(self, target_sample_rate):
@@ -154,3 +213,42 @@ class AudioSegment:
             st, ed = a * hop, min(b * hop, n)
             out.append({'start': st / sr, 'end': ed / sr} if return_seconds else {'start': st, 'end': ed})
         return out
+
+
+class FlacSegment(AudioSegment):
+    """A native FLAC stream: ``sample_rate`` and ``duration`` come from STREAMINFO without decoding; ``samples`` are
+    decoded on the current CUDA device (vp_flac_decode) the first time they are read, and ``decode_device`` gives them
+    as a device row without a host copy.  ``name`` labels the stream in errors."""
+
+    def __init__(self, data, name='<flac>'):
+        from .flac import parse_streaminfo
+        self.data = bytes(data)
+        self.info = parse_streaminfo(self.data)
+        self.name = str(name)
+        self.sample_rate = self.info.sample_rate
+        self._samples = None
+
+    @property
+    def samples(self):
+        if self._samples is None:
+            decode_segments([self])
+        return self._samples
+
+    @samples.setter
+    def samples(self, value):
+        self._samples = value
+
+    @property
+    def duration(self):
+        if self._samples is None:
+            return self.info.duration
+        return self._samples.shape[0] / float(self.sample_rate)
+
+    def decode_device(self, engine):
+        """The decoded stream as a CUDA float32 row [total_samples] on ``engine``'s device (ValueError when refused);
+        the row is kept, so a second call on the same device decodes nothing."""
+        row = getattr(self, '_device_row', None)
+        if row is None or row.device != engine.device:
+            rows, _ = engine.decode_flac([self.data], [self.info], [self.name])
+            self._device_row = row = rows[0]
+        return row

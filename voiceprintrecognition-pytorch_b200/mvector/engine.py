@@ -187,6 +187,44 @@ class Engine:
         _check(self._h, L.lib().vp_gather_windows(self._h, C.c_void_p(src.data_ptr()), C.c_void_p(offset.data_ptr()),
                                                   C.c_void_p(valid.data_ptr()), n, int(ld), C.c_void_p(dst.data_ptr()), sp))
 
+    # ---- FLAC decoding (csrc/flac.cu) ----
+    def decode_flac(self, streams, infos=None, names=None, ld=None, check=True):
+        """Native FLAC streams (bytes-like each; ``infos`` their flac.StreamInfo, parsed here when omitted) -> (rows CUDA
+        float32 [B, ld] at the native rates, zero filled past each stream's length, status CUDA int32 [B]): one
+        vp_flac_decode, every row mixed to mono exactly as audio.pcm_to_mono mixes the same integers.  ``ld`` defaults to
+        the longest stream.  With ``check`` a non-zero status raises ValueError naming the item (``names``, default
+        'item i'); that waits for the decode."""
+        from .flac import FlacBatch, check_status, parse_streaminfo
+        infos = [parse_streaminfo(s) for s in streams] if infos is None else list(infos)
+        batch = FlacBatch(streams, infos, self.device, names)
+        B = len(batch)
+        ld = int(batch.lengths.max()) if ld is None and B else int(ld or 0)
+        out = torch.empty(B, ld, dtype=torch.float32, device=self.device)
+        status = torch.empty(B, dtype=torch.int32, device=self.device)
+        self.decode_flac_into(batch, out, ld, status)
+        if check:
+            check_status(status.cpu().numpy(), batch.names)
+        return out, status
+
+    def decode_flac_into(self, batch, out, ld, status, stream=None):
+        """vp_flac_decode of a flac.FlacBatch into ``out``, contiguous CUDA float32 holding B rows of ``ld`` (a matrix or a
+        flat staging slot), and the int32 ``status`` on ``stream`` (default: the current stream)."""
+        B = len(batch)
+        if B == 0:
+            return
+        assert out.dtype == torch.float32 and out.is_cuda and out.is_contiguous() and out.numel() >= B * ld
+        assert status.dtype == torch.int32 and status.is_cuda and status.numel() >= B
+        stream = torch.cuda.current_stream(self.device) if stream is None else stream
+        with torch.cuda.stream(stream):              # the scratch belongs to the stream the decode runs on
+            scratch = torch.empty(max(int(L.lib().vp_flac_scratch_bytes(self._h, B, batch.nbytes, batch.max_frames)), 1),
+                                  dtype=torch.uint8, device=self.device)
+        sp = C.c_void_p(stream.cuda_stream)
+        _check(self._h, L.lib().vp_flac_decode(
+            self._h, C.c_void_p(batch.data.data_ptr()), C.c_void_p(batch.stream_off_dev.data_ptr()),
+            C.c_void_p(batch.frame_off_dev.data_ptr()), C.c_void_p(batch.info.data_ptr()), B,
+            C.c_void_p(out.data_ptr()), int(ld), C.c_void_p(status.data_ptr()), C.c_void_p(scratch.data_ptr()),
+            batch.nbytes, batch.max_frames, sp))
+
     # ---- verification metrics (csrc/verify.cu) ----
     def verify(self, scores, labels=None, trial_labels=None, enroll_labels=None, p_target=0.01, c_miss=1, c_fa=1,
                sorted_out=False):

@@ -25,7 +25,7 @@ import torch
 import yaml
 from loguru import logger
 
-from .audio import AudioSegment
+from .audio import AudioSegment, FlacSegment, decode_segments, device_samples
 from .data_utils.featurizer import AudioFeaturizer
 from .engine import Engine
 from .infer_utils.speaker_diarization import SpeakerDiarization
@@ -301,8 +301,9 @@ class MVectorPredictor:
         return out
 
     def _embed_waves(self, waves, lmax, masked, to_numpy=True, group=None, rates=None):
-        """waves: list of 1-D float32 arrays, decoded, at ``rates`` Hz (None: all at the model's rate), or DeviceWindows
-        (rows already on the device) -> [B, embd_dim] (np.float32, or the device tensor with ``to_numpy=False``).
+        """waves: list of 1-D float32 arrays, decoded, at ``rates`` Hz (None: all at the model's rate), or a device-rows
+        object (DeviceWindows, flac.DeviceFlacRows: ``lens``, ``gather``, ``check``, rows written on the device)
+        -> [B, embd_dim] (np.float32, or the device tensor with ``to_numpy=False``).
         ``lmax`` is the longest item AFTER resampling.
 
         Conditioning (predict.py:205-211) runs on the device inside the staging: a stage with rows to resample is
@@ -320,8 +321,9 @@ class MVectorPredictor:
         slices finish (``vp_host_stage_h2d``) -- feed the fused front-end kernels, which run on the main stream behind an
         event of their stage's copies and write straight into the [B, T, F] feature buffer; as soon as the features of a
         backbone chunk (``_host_chunks``) are complete the main stream runs its program, under the next stage's gather and
-        copies.  With DeviceWindows a stage's rows are written into its device slot by vp_gather_windows on the copy
-        stream instead; everything after that is the same.  One D2H of the result at the end."""
+        copies.  With device rows a stage's rows are written into its device slot on the copy stream instead -- by
+        vp_gather_windows (DeviceWindows) or vp_flac_decode (DeviceFlacRows) -- and everything after that is the same.
+        One D2H of the result at the end; a refused FLAC stream raises ValueError after it."""
         from . import _lib as L
         import ctypes as C
         import time
@@ -343,8 +345,8 @@ class MVectorPredictor:
         lib = L.lib()
         F = fz.feature_dim
         ds_conf = self.configs.dataset_conf.dataset
-        dev_rows = isinstance(waves, DeviceWindows)
-        lens = np.full(B, waves.size, dtype=np.int32) if dev_rows else np.fromiter(map(len, waves), dtype=np.int32, count=B)
+        dev_rows = hasattr(waves, 'gather')              # DeviceWindows / DeviceFlacRows: rows written on the device
+        lens = np.asarray(waves.lens, dtype=np.int32) if dev_rows else np.fromiter(map(len, waves), dtype=np.int32, count=B)
         plan = None
         gain_db = ds_conf.target_dB if ds_conf.use_dB_normalization else None
         if gain_db is not None or (rates is not None and any(int(r) != ds_conf.sample_rate for r in rates)):
@@ -370,9 +372,7 @@ class MVectorPredictor:
                 flags = torch.empty(B, dtype=torch.int32, device=dev)
                 gscratch = plan.scratch(S, lmax)
         scratch = torch.empty(max(int(lib.vp_frontend_scratch_floats(eng.handle, S, lmax)), 1), dtype=torch.float32, device=dev)
-        if self._copy_stream is None:
-            self._copy_stream = torch.cuda.Stream(device=dev)
-        cs = self._copy_stream
+        cs = self._staging_stream()
         cs_ptr = C.c_void_p(cs.cuda_stream)
         main = torch.cuda.current_stream(dev)
         main_ptr = C.c_void_p(main.cuda_stream)
@@ -405,7 +405,7 @@ class MVectorPredictor:
             dst = dnat[ds] if resample else dw
             if dev_rows:
                 waves.gather(g0, g1, dst, ld, cs)
-                mark(f'stage {gi}: {n} windows gathered on the device')
+                mark(f'stage {gi}: {n} rows written on the device')
             else:
                 if pin_ev[ps] is not None:
                     pin_ev[ps].synchronize()
@@ -447,6 +447,8 @@ class MVectorPredictor:
         main.wait_stream(cs)
         mark('all kernels enqueued')
         out = emb.cpu().numpy() if to_numpy else emb
+        if dev_rows:
+            waves.check()                               # a refused FLAC stream: after the result copy
         if flags is not None:
             plan.check(flags.cpu().numpy(), waves)      # after the result copy: no extra synchronise
         mark('result on host' if to_numpy else 'returned device tensor')
@@ -491,14 +493,14 @@ class MVectorPredictor:
     def predict(self, audio_data, sample_rate=16000):
         """预测一个音频的特征 (predict.py:214-229) -> np.ndarray [embd_dim]"""
         seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
-        w = np.ascontiguousarray(seg.samples, dtype=np.float32)
-        lmax = int(self._output_lengths([w.shape[0]], [seg.sample_rate])[0])
-        return self._embed_waves([w], lmax, masked=False, rates=[seg.sample_rate])[0]
+        waves = self._flac_rows([seg]) or [np.ascontiguousarray(seg.samples, dtype=np.float32)]
+        lmax = int(self._output_lengths(self._row_lengths(waves), [seg.sample_rate])[0])
+        return self._embed_waves(waves, lmax, masked=False, rates=[seg.sample_rate])[0]
 
     def predict_batch(self, audios_data, sample_rate=16000, batch_size=32):
         """预测一批音频的特征 (predict.py:231-265) -> np.ndarray [B, embd_dim], order preserved."""
         waves, rates = self._load_batch(audios_data, sample_rate)
-        lmax = int(self._output_lengths(list(map(len, waves)), rates).max()) if waves else 0
+        lmax = int(self._output_lengths(self._row_lengths(waves), rates).max()) if len(waves) else 0
         return self._embed_waves(waves, lmax, masked=True, rates=rates)
 
     def _output_lengths(self, n_in, rates):
@@ -519,7 +521,30 @@ class MVectorPredictor:
             if len(audios_data) == 0 or shortest / float(sample_rate) >= ds.min_duration:
                 return list(audios_data), [int(sample_rate)] * len(audios_data)
         segs = [self._load_audio(audio_data=a, sample_rate=sample_rate) for a in audios_data]
+        rows = self._flac_rows(segs)
+        if rows is not None:
+            return rows, [s.sample_rate for s in segs]
+        decode_segments(segs, self._audio_featurizer.engine)   # a mixed list: its FLAC items in one device decode
         return [np.ascontiguousarray(s.samples, dtype=np.float32) for s in segs], [s.sample_rate for s in segs]
+
+    def _flac_rows(self, segs):
+        """DeviceFlacRows of ``segs`` when every one is an undecoded FLAC segment (their compressed bytes go up in one
+        pinned copy on the copy stream and each stage decodes into its slot), else None."""
+        if not segs or not all(isinstance(s, FlacSegment) and s._samples is None for s in segs):
+            return None
+        from .flac import DeviceFlacRows
+        return DeviceFlacRows(self._audio_featurizer.engine, segs, self._staging_stream())
+
+    @staticmethod
+    def _row_lengths(waves):
+        """Native sample count of every row: host arrays or a device-rows object (``lens``)."""
+        return waves.lens if hasattr(waves, 'lens') else list(map(len, waves))
+
+    def _staging_stream(self):
+        """The copy stream the staging of ``_embed_waves`` issues its uploads on."""
+        if self._copy_stream is None:
+            self._copy_stream = torch.cuda.Stream(device=self.device)
+        return self._copy_stream
 
     def contrast(self, audio_data1, audio_data2):
         """声纹对比 (predict.py:267-279) -> cosine similarity"""
@@ -529,7 +554,9 @@ class MVectorPredictor:
 
     def register(self, audio_data, user_name: str, sample_rate=16000):
         """声纹注册 (predict.py:281-309)"""
-        seg = self._condition_host(self._load_audio(audio_data=audio_data, sample_rate=sample_rate))
+        seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
+        decode_segments([seg], self._audio_featurizer.engine)   # a FLAC file: decoded with this predictor's engine
+        seg = self._condition_host(seg)
         feature = self.predict(audio_data=seg.samples, sample_rate=seg.sample_rate)
         if self.audio_feature is None:
             self.audio_feature = feature
@@ -587,14 +614,14 @@ class MVectorPredictor:
         seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
         ds = self.configs.dataset_conf.dataset
         eng = self._engine
-        x = torch.from_numpy(np.ascontiguousarray(seg.samples, dtype=np.float32)).to(self.device)
+        x = device_samples(seg, eng)                       # a FLAC recording is decoded on the device
         gain_db = ds.target_dB if ds.use_dB_normalization else None
         y, n_out, flags = eng.condition(x.view(1, -1), [x.numel()], [seg.sample_rate], ds.sample_rate, gain_db)
         n, sr = int(n_out[0]), int(ds.sample_rate)
         y = y.view(-1)
         energy = eng.frame_energy(y, n, AudioSegment.vad_hop(sr)).cpu().numpy()
         if flags is not None and flags.cpu().numpy().any():  # a silent recording: _condition_host's ValueError
-            eng.condition_plan([x.numel()], [seg.sample_rate], sr, gain_db).check(flags.cpu().numpy(), [seg.samples])
+            eng.condition_plan([x.numel()], [seg.sample_rate], sr, gain_db).check(flags.cpu().numpy(), [x.cpu().numpy()])
         table = self.speaker_diarize.chunk_table(AudioSegment.vad_from_energy(energy, n, sr, return_seconds=True), n, sr)
         # the chunks go on with the caller's sample_rate, as in the reference (predict.py:379): a caller at another rate
         # has them resampled a second time, and predict_batch's too-short assert applies to each of them
@@ -620,6 +647,7 @@ class DeviceWindows:
     def __init__(self, engine, src, table):
         self.engine, self.src, self.table = engine, src, table
         self.size = int(table.size)
+        self.lens = np.full(len(table.start), self.size, dtype=np.int32)
         self._offset = torch.from_numpy(table.offset).to(src.device)
         self._valid = torch.from_numpy(table.valid).to(src.device)
 
@@ -636,3 +664,6 @@ class DeviceWindows:
     def gather(self, lo, hi, dst, ld, stream):
         """Rows lo..hi into the device slot ``dst`` [hi - lo, ld] on ``stream``."""
         self.engine.gather_windows(self.src, self._offset[lo:hi], self._valid[lo:hi], ld, dst, stream)
+
+    def check(self):
+        """Nothing to report: a window of a decoded recording cannot fail."""

@@ -25,7 +25,7 @@ import torch
 import yaml
 from loguru import logger
 
-from .audio import AudioSegment
+from .audio import AudioSegment, FlacSegment, device_samples
 from .data_utils.featurizer import AudioFeaturizer
 from .metric.metrics import compute_dcf, compute_eer, compute_fnr_fpr
 from .utils.utils import dict_to_object, print_arguments
@@ -74,6 +74,8 @@ class MVectorTrainer(object):
                         try:
                             cand = AudioSegment.from_file(path)
                             if cand.duration >= min_duration:
+                                if isinstance(cand, FlacSegment):      # a corrupt FLAC file is skipped like a bad WAV
+                                    cand.decode_device(self.audio_featurizer.engine)
                                 seg = cand
                                 break
                         except Exception as e:  # noqa: BLE001  (the reference logs and moves on, reader.py:103-106)
@@ -155,7 +157,7 @@ class MVectorTrainer(object):
             n = seg.samples.shape[0]
             crop = int(max_duration * sample_rate) if n / float(sample_rate) > max_duration else n
             return torch.from_numpy(seg.samples[:crop])
-        x = torch.from_numpy(np.ascontiguousarray(seg.samples, dtype=np.float32)).to(eng.device)
+        x = device_samples(seg, eng)                           # a FLAC file is decoded on the device
         n = x.shape[0]
         if seg.sample_rate != sample_rate or target_db is not None:
             y, n_out, flags = eng.condition(x.unsqueeze(0), [n], [seg.sample_rate], sample_rate, target_db)
