@@ -265,7 +265,9 @@ int vp_device_zero(void* device_ptr, size_t nbytes, void* stream);
 /* Cosine score matrix scores[i, j] = <a_i, b_j> / (|a_i| |b_j|), a [n, D], b [m, D], scores [n, m] (device, row-major):
  * the scoring step of the callers around the embedding path -- retrieval against the enrolled speaker means
  * (predict.py:169-183), evaluate's trial-vs-enrol scores (trainer.py:454-461) and the diarization similarity matrix
- * (infer_utils/speaker_diarization.py:254-257). */
+ * (infer_utils/speaker_diarization.py:254-257).  A zero-norm row scores +0 against every row, itself included, as
+ * sklearn's cosine_similarity normalises a zero row to zero; a row holding a NaN gives NaN in its own row or column
+ * only.  Any n, m, D >= 1; a score depends only on its two rows, not on n, m or its place in the matrix. */
 int vp_cosine_scores(vp_handle* h, const float* a, int32_t n, const float* b, int32_t m, int32_t D, float* scores, void* stream);
 
 /* ------------------------------------------------------------------------------------------------------------

@@ -385,52 +385,61 @@ cudaError_t launch_pool2d(const PoolParams& p, cudaStream_t stream) {
 }  // namespace vpb
 
 // ---------------------------------------------------------------------------------------------------------------
-// Cosine score matrix  out[i, j] = <a_i, b_j> / (|a_i| |b_j|)  for a [n, D], b [m, D] (row-major, D % 4 == 0):
+// Cosine score matrix  out[i, j] = <a_i, b_j> / (|a_i| |b_j|)  for a [n, D], b [m, D] (row-major, any D >= 1):
 // the scoring half of the callers around the embedding path -- voiceprint retrieval against the enrolled means
 // (predict.py:169-183), trial-vs-enrol scoring of evaluate (trainer.py:454-461, sklearn cosine_similarity) and the
 // similarity matrix of the diarization clustering (speaker_diarization.py:254-257).  One CTA = 32 x 32 scores, the two
 // row blocks staged through shared memory in K chunks of 64, norms accumulated from the same tiles; fixed summation
-// order -> deterministic.
+// order -> deterministic, and a score does not depend on where its pair sits in the matrix.
+// A zero-norm row scores 0 against everything, as sklearn's normalize() leaves a zero row zero: its norm is taken as 1,
+// and its dot products are +0.  The CTAs of one grid row walk the tile rows with a stride of gridDim.y, which is capped
+// at 65535, so every n and m up to INT32_MAX launches.
 // ---------------------------------------------------------------------------------------------------------------
 namespace vpb {
+
+constexpr int COS_GRID_Y_MAX = 65535;
 
 __global__ void __launch_bounds__(256) cosine_scores_kernel(const float* __restrict__ a, const float* __restrict__ b, float* __restrict__ out,
                                                             int n, int m, int D, int a_ld, int b_ld, int out_ld) {
   __shared__ float sa[32][65], sb[32][65];
   const int tx = threadIdx.x & 31, ty = threadIdx.x >> 5;            // thread -> column j = tx, rows ty, ty+8, ty+16, ty+24
-  const int i0 = blockIdx.y * 32, j0 = blockIdx.x * 32;
-  float dot[4] = {0.f, 0.f, 0.f, 0.f}, na[4] = {0.f, 0.f, 0.f, 0.f}, nb = 0.f;
-  for (int k0 = 0; k0 < D; k0 += 64) {
-    for (int e = threadIdx.x; e < 32 * 64; e += 256) {
-      const int r = e >> 6, c = e & 63;
-      sa[r][c] = (i0 + r < n && k0 + c < D) ? __ldg(a + (size_t)(i0 + r) * a_ld + k0 + c) : 0.f;
-      sb[r][c] = (j0 + r < m && k0 + c < D) ? __ldg(b + (size_t)(j0 + r) * b_ld + k0 + c) : 0.f;
-    }
-    __syncthreads();
+  const int j0 = blockIdx.x * 32;
+  for (long long i0 = (long long)blockIdx.y * 32; i0 < n; i0 += (long long)gridDim.y * 32) {
+    float dot[4] = {0.f, 0.f, 0.f, 0.f}, na[4] = {0.f, 0.f, 0.f, 0.f}, nb = 0.f;
+    for (int k0 = 0; k0 < D; k0 += 64) {
+      for (int e = threadIdx.x; e < 32 * 64; e += 256) {
+        const int r = e >> 6, c = e & 63;
+        sa[r][c] = (i0 + r < n && k0 + c < D) ? __ldg(a + (size_t)(i0 + r) * a_ld + k0 + c) : 0.f;
+        sb[r][c] = (j0 + r < m && k0 + c < D) ? __ldg(b + (size_t)(j0 + r) * b_ld + k0 + c) : 0.f;
+      }
+      __syncthreads();
 #pragma unroll 8
-    for (int c = 0; c < 64; ++c) {
-      const float bv = sb[tx][c];
-      nb = fmaf(bv, bv, nb);
+      for (int c = 0; c < 64; ++c) {
+        const float bv = sb[tx][c];
+        nb = fmaf(bv, bv, nb);
+#pragma unroll
+        for (int q = 0; q < 4; ++q) {
+          const float av = sa[ty + 8 * q][c];
+          dot[q] = fmaf(av, bv, dot[q]);
+          na[q] = fmaf(av, av, na[q]);
+        }
+      }
+      __syncthreads();
+    }
+    const int j = j0 + tx;
+    const float rb = nb == 0.f ? 1.f : sqrtf(nb);
+    if (j < m)
 #pragma unroll
       for (int q = 0; q < 4; ++q) {
-        const float av = sa[ty + 8 * q][c];
-        dot[q] = fmaf(av, bv, dot[q]);
-        na[q] = fmaf(av, av, na[q]);
+        const long long i = i0 + ty + 8 * q;
+        if (i < n) out[(size_t)i * out_ld + j] = dot[q] / ((na[q] == 0.f ? 1.f : sqrtf(na[q])) * rb);
       }
-    }
-    __syncthreads();
   }
-  const int j = j0 + tx;
-  if (j < m)
-#pragma unroll
-    for (int q = 0; q < 4; ++q) {
-      const int i = i0 + ty + 8 * q;
-      if (i < n) out[(size_t)i * out_ld + j] = dot[q] / (sqrtf(na[q]) * sqrtf(nb));
-    }
 }
 
 cudaError_t launch_cosine_scores(const float* a, const float* b, float* out, int n, int m, int D, cudaStream_t stream) {
-  dim3 grid((m + 31) / 32, (n + 31) / 32);
+  const long long tiles_n = (n + 31LL) / 32;
+  dim3 grid((unsigned)((m + 31LL) / 32), (unsigned)(tiles_n < COS_GRID_Y_MAX ? tiles_n : COS_GRID_Y_MAX));
   cosine_scores_kernel<<<grid, 256, 0, stream>>>(a, b, out, n, m, D, D, D, m);
   return cudaGetLastError();
 }
