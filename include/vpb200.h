@@ -422,6 +422,40 @@ int vp_flac_decode(vp_handle* h, const uint8_t* data, const int64_t* stream_off,
                    const vp_flac_info* info, int32_t B, float* out, int64_t ld, int32_t* status, void* scratch,
                    int64_t nbytes, int64_t max_frames, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Uncompressed PCM containers (WAV, WAVE_FORMAT_EXTENSIBLE, RF64 / BW64, AIFF / AIFF-C): B rows of raw interleaved
+ * samples converted on the device.  mvector/pcm.py parses the headers on the host; the device reads only sample bytes.
+ * Row b is float32 mono at the file's native rate, bit-identical to mvector.pcm.to_mono:
+ *   integers of container width N bits (U8 is WAV's unsigned 8-bit, S8 AIFF's signed): x / 2^(N-1) in float32, exactly
+ *     mvector.audio.pcm_to_mono (32-bit: float32(x) rounded to nearest first);
+ *   F32: the stored value, no scaling or clipping; F64: rounded to nearest float32;
+ *   ULAW / ALAW: the ITU-T G.711 expansion to a 16-bit integer (extremes +-32124 / +-32256), then / 2^15;
+ *   channels 1..8: numpy's float32 mean -- left to right below 8 channels, ((c0+c1)+(c2+c3))+((c4+c5)+(c6+c7)) for 8,
+ *     then one division by the count (the order vp_flac_decode uses).
+ * ---------------------------------------------------------------------------------------------------------- */
+enum {
+  VP_PCM_U8 = 1, VP_PCM_S8 = 2, VP_PCM_S16LE = 3, VP_PCM_S16BE = 4, VP_PCM_S24LE = 5, VP_PCM_S24BE = 6,
+  VP_PCM_S32LE = 7, VP_PCM_S32BE = 8, VP_PCM_F32LE = 9, VP_PCM_F32BE = 10, VP_PCM_F64LE = 11, VP_PCM_F64BE = 12,
+  VP_PCM_ULAW = 13, VP_PCM_ALAW = 14
+};
+typedef struct vp_pcm_info {  /* where a row's samples are and how they are stored */
+  int64_t byte_off;            /* offset of the first sample byte in data */
+  int64_t frames;              /* samples per channel, 0..ld */
+  int32_t channels;            /* 1..8, interleaved */
+  int32_t format;              /* VP_PCM_* */
+  int32_t reserved0;
+  int32_t reserved1;
+} vp_pcm_info;
+int32_t vp_sizeof_pcm_info(void);    /* binding self-check: sizeof(vp_pcm_info) */
+/* data: nbytes bytes (device, any alignment; may be null when nbytes is 0); info [B] (device); B in [0, 65535].
+ * out [B, ld] float32 (device; may be null when ld is 0): row b at out + b * ld <- its frames converted as above, zero filled from frames to ld.
+ * status int32 [B] (device) <- 0, or an OR of reasons checked before any of the row's bytes is read: 1 unknown format,
+ * 2 channels outside 1..8, 4 frames outside [0, ld], 8 sample bytes [byte_off, byte_off + frames * channels * width)
+ * not inside [0, nbytes).  A refused row is written as zeros; the other rows are exact.  Every read of a row stays
+ * inside its own sample bytes.  Asynchronous on stream. */
+int vp_pcm_decode(vp_handle* h, const uint8_t* data, int64_t nbytes, const vp_pcm_info* info, int32_t B, float* out,
+                  int64_t ld, int32_t* status, void* stream);
+
 /* Staging half of predict_batch (predict.py:244-255) as ONE native call: worker threads gather slices of slice_rows
  * utterances into the zero-padded PINNED matrix staging[n, lmax]; the calling thread -- one of the n_threads gatherers --
  * issues cudaMemcpyAsync(staging slice -> device_dst slice) on copy_stream, in slice order, as soon as a slice is

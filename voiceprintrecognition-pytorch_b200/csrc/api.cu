@@ -991,6 +991,21 @@ int vp_flac_decode(vp_handle* h, const uint8_t* data, const int64_t* stream_off,
   return VP_OK;
 }
 
+int32_t vp_sizeof_pcm_info(void) { return (int32_t)sizeof(vp_pcm_info); }
+
+int vp_pcm_decode(vp_handle* h, const uint8_t* data, int64_t nbytes, const vp_pcm_info* info, int32_t B, float* out,
+                  int64_t ld, int32_t* status, void* stream) {
+  if (!h) return VP_ERR_INVALID;
+  if (B < 0 || B > 65535) return fail(h, VP_ERR_UNSUPPORTED, "B = %d outside [0, 65535]", B);
+  if (B == 0) return VP_OK;
+  if (nbytes < 0 || ld < 0)
+    return fail(h, VP_ERR_INVALID, "nbytes = %lld, ld = %lld: negative", (long long)nbytes, (long long)ld);
+  if ((nbytes && !data) || !info || (ld && !out) || !status) return fail(h, VP_ERR_INVALID, "null argument");
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  CUDA_TRY(h, launch_pcm_decode(data, nbytes, info, B, out, ld, status, (cudaStream_t)stream));
+  return VP_OK;
+}
+
 int vp_program_peek(vp_program* p, int64_t off, size_t nbytes, void* dst, void* stream) {
   if (!p || !dst) return VP_ERR_INVALID;
   if (off < 0 || (size_t)off + nbytes > p->ws_bytes) return fail(p->h, VP_ERR_INVALID, "peek out of range");

@@ -102,6 +102,10 @@ cudaError_t launch_flac_decode(const uint8_t* data, int64_t nbytes, const int64_
                                const vp_flac_info* info, int B, int64_t max_frames, float* out, int64_t ld,
                                int32_t* status, void* scratch, cudaStream_t stream);
 
+// PCM container samples -> float32 mono rows (pcm.cu)
+cudaError_t launch_pcm_decode(const uint8_t* data, int64_t nbytes, const vp_pcm_info* info, int B, float* out,
+                              int64_t ld, int32_t* status, cudaStream_t stream);
+
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);

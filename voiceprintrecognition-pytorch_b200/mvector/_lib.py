@@ -60,6 +60,11 @@ class FlacInfo(C.Structure):
                 ('max_framesize', C.c_int32), ('reserved0', C.c_int32)]
 
 
+class PcmInfo(C.Structure):
+    _fields_ = [('byte_off', C.c_int64), ('frames', C.c_int64), ('channels', C.c_int32), ('format', C.c_int32),
+                ('reserved0', C.c_int32), ('reserved1', C.c_int32)]
+
+
 class VpError(RuntimeError):
     def __init__(self, code, msg):
         super().__init__(f'vpb200 error {code}: {msg}')
@@ -133,6 +138,8 @@ def lib():
         'vp_flac_scratch_bytes': (sz, [vp, i32, C.c_int64, C.c_int64]),
         'vp_flac_decode': (C.c_int, [vp, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, i32, f32p, C.c_int64,
                                      C.c_void_p, C.c_void_p, C.c_int64, C.c_int64, vp]),
+        'vp_sizeof_pcm_info': (i32, []),
+        'vp_pcm_decode': (C.c_int, [vp, C.c_void_p, C.c_int64, C.c_void_p, i32, f32p, C.c_int64, C.c_void_p, vp]),
     }
     for name, (res, args) in sig.items():
         fn = getattr(L, name)          # AttributeError here = header/library mismatch
@@ -141,8 +148,10 @@ def lib():
     if L.vp_abi_version() != 4:
         raise RuntimeError('libvpb200.so ABI version mismatch')
     if L.vp_sizeof_op() != C.sizeof(Op) or L.vp_sizeof_frontend_desc() != C.sizeof(FrontendDesc) \
-            or L.vp_sizeof_frontend_options() != C.sizeof(FrontendOptions) or L.vp_sizeof_flac_info() != C.sizeof(FlacInfo):
-        raise RuntimeError('vp_op / vp_frontend_desc / vp_frontend_options / vp_flac_info layout mismatch between the ctypes binding '
+            or L.vp_sizeof_frontend_options() != C.sizeof(FrontendOptions) or L.vp_sizeof_flac_info() != C.sizeof(FlacInfo) \
+            or L.vp_sizeof_pcm_info() != C.sizeof(PcmInfo):
+        raise RuntimeError('vp_op / vp_frontend_desc / vp_frontend_options / vp_flac_info / vp_pcm_info layout mismatch '
+                           'between the ctypes binding '
                            'and libvpb200.so')
     _lib = L
     return L
@@ -157,4 +166,4 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
            'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics',
            'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize', 'vp_frame_energy', 'vp_gather_windows',
-           'vp_sizeof_flac_info', 'vp_flac_scratch_bytes', 'vp_flac_decode']
+           'vp_sizeof_flac_info', 'vp_flac_scratch_bytes', 'vp_flac_decode', 'vp_sizeof_pcm_info', 'vp_pcm_decode']

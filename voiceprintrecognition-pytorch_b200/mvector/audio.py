@@ -2,9 +2,13 @@
 ``samples`` (float32 mono in [-1, 1]), ``sample_rate``, ``duration``, ``from_file`` / ``from_ndarray`` / ``from_bytes``,
 ``resample``, ``normalize``, ``vad``.  yeaudio (requirements.txt:12) is a third-party package absent from the reference tree and
 from this image; decoding/resampling sit OUTSIDE the parity boundary (SURVEY.md 8a3: parity starts at identical
-waveforms).  Decoding covers PCM WAV via the standard library and native FLAC (RFC 9639) on the device: a FLAC segment
-knows its rate and duration from STREAMINFO and is decoded by vp_flac_decode the first time its samples are read.  Both
-formats turn their integers into float32 mono with ``pcm_to_mono``."""
+waveforms).  Decoding covers the uncompressed PCM containers -- WAV (integer, float, A-law and mu-law, also
+WAVE_FORMAT_EXTENSIBLE), RF64 / BW64 and AIFF / AIFF-C -- and native FLAC (RFC 9639).  Either segment knows its rate and
+duration from the header alone.  A FLAC segment is decoded by vp_flac_decode the first time its samples are read; a PCM
+segment's samples are converted by numpy on first read (pcm.to_mono), and both give a device row without a host copy
+(``decode_device``: vp_flac_decode / vp_pcm_decode).  Integers become float32 mono with ``pcm_to_mono``; pcm.py states
+the rule for floats and G.711.  Other input, and a RIFF file the PCM parser refuses, still goes to the standard
+library's ``wave`` reader."""
 import io
 import os
 import wave
@@ -67,10 +71,10 @@ def _engine(device=None):
 
 
 def device_samples(seg, engine):
-    """A segment's samples as a CUDA float32 row on ``engine``'s device: an undecoded FLAC segment is decoded there and
-    its PCM never visits the host; any other segment's samples are uploaded."""
+    """A segment's samples as a CUDA float32 row on ``engine``'s device: an undecoded FLAC or PCM segment is converted
+    there from its file's bytes and its samples never visit the host; any other segment's samples are uploaded."""
     import torch
-    if isinstance(seg, FlacSegment) and seg._samples is None:
+    if isinstance(seg, (FlacSegment, PcmSegment)) and seg._samples is None:
         return seg.decode_device(engine)
     return torch.from_numpy(np.ascontiguousarray(seg.samples, dtype=np.float32)).to(engine.device)
 
@@ -124,25 +128,47 @@ class AudioSegment:
 
     @classmethod
     def from_file(cls, file):
-        """A WAV or native FLAC file (path or binary file object), told apart by the FLAC magic."""
+        """A PCM container or native FLAC file (path or binary file object), told apart by its magic; anything else is
+        read by ``wave``."""
         from .flac import is_flac
+        from .pcm import is_pcm
         if isinstance(file, (str, os.PathLike)):
             with open(file, 'rb') as f:
-                if not is_flac(f.read(4)):
+                head = f.read(4)
+                if not (is_flac(head) or is_pcm(head)):
                     return cls._from_wave(file)
                 f.seek(0)
-                return FlacSegment(f.read(), name=os.fspath(file))
-        data = file.read()
-        if is_flac(data):
-            return FlacSegment(data, name=getattr(file, 'name', '<file>'))
-        return cls._from_wave(io.BytesIO(data))
+                return cls._from_data(f.read(), os.fspath(file))
+        return cls._from_data(file.read(), getattr(file, 'name', '<file>'))
 
     @classmethod
     def from_bytes(cls, data):
+        return cls._from_data(data, '<bytes>')
+
+    @classmethod
+    def _from_data(cls, data, name):
         from .flac import is_flac
+        from .pcm import is_pcm
         if is_flac(data):
-            return FlacSegment(data, name='<bytes>')
+            return FlacSegment(data, name=name)
+        if is_pcm(data):
+            return cls._from_pcm(data, name)
         return cls._from_wave(io.BytesIO(data))
+
+    @classmethod
+    def _from_pcm(cls, data, name):
+        """A PcmSegment; or, for a RIFF file the PCM parser refuses but the ``wave`` reader reads (integer PCM of more
+        than 8 channels, a block align that contradicts the format), the segment the ``wave`` reader gives, as it did
+        before the parser existed.  When neither reads the file, the parser's error is raised."""
+        try:
+            return PcmSegment(data, name=name)
+        except (ValueError, NotImplementedError) as err:
+            if bytes(data[:4]) != b'RIFF':
+                raise
+            try:
+                return AudioSegment._from_wave(io.BytesIO(data))
+            except Exception:  # noqa: BLE001  (the wave reader's own error says less than the parser's)
+                raise err from None
 
     def resample(self, target_sample_rate):
         if target_sample_rate == self.sample_rate:
@@ -250,5 +276,46 @@ class FlacSegment(AudioSegment):
         row = getattr(self, '_device_row', None)
         if row is None or row.device != engine.device:
             rows, _ = engine.decode_flac([self.data], [self.info], [self.name])
+            self._device_row = row = rows[0]
+        return row
+
+
+class PcmSegment(AudioSegment):
+    """An uncompressed PCM container file (WAV, RF64 / BW64, AIFF / AIFF-C): ``sample_rate`` and ``duration`` come from
+    the header without converting; ``samples`` are converted on the host by numpy (pcm.to_mono) the first time they are
+    read, and ``decode_device`` converts the file's bytes on the device (vp_pcm_decode) into the same row.  ``name``
+    labels the file in errors."""
+
+    def __init__(self, data, name='<pcm>'):
+        from .pcm import parse_header
+        self.data = bytes(data)
+        self.info = parse_header(self.data)
+        self.name = str(name)
+        self.sample_rate = self.info.sample_rate
+        self._samples = None
+
+    @property
+    def samples(self):
+        if self._samples is None:
+            from .pcm import to_mono
+            self._samples = to_mono(self.data, self.info)
+        return self._samples
+
+    @samples.setter
+    def samples(self, value):
+        self._samples = value
+
+    @property
+    def duration(self):
+        if self._samples is None:
+            return self.info.duration
+        return self._samples.shape[0] / float(self.sample_rate)
+
+    def decode_device(self, engine):
+        """The converted file as a CUDA float32 row [frames] on ``engine``'s device; the row is kept, so a second call on
+        the same device converts nothing."""
+        row = getattr(self, '_device_row', None)
+        if row is None or row.device != engine.device:
+            rows, _ = engine.decode_pcm([self.data], [self.info], [self.name])
             self._device_row = row = rows[0]
         return row

@@ -225,6 +225,38 @@ class Engine:
             C.c_void_p(out.data_ptr()), int(ld), C.c_void_p(status.data_ptr()), C.c_void_p(scratch.data_ptr()),
             batch.nbytes, batch.max_frames, sp))
 
+    # ---- PCM container conversion (csrc/pcm.cu) ----
+    def decode_pcm(self, files, infos=None, names=None, ld=None, check=True):
+        """Uncompressed PCM container files (bytes-like each; ``infos`` their pcm.PcmInfo, parsed here when omitted) ->
+        (rows CUDA float32 [B, ld] at the native rates, zero filled past each file's length, status CUDA int32 [B]): one
+        vp_pcm_decode, every row bit-identical to pcm.to_mono.  ``ld`` defaults to the longest file.  With ``check`` a
+        non-zero status raises ValueError naming the item (``names``, default 'item i'); that waits for the
+        conversion."""
+        from .pcm import PcmBatch, check_status, parse_header
+        infos = [parse_header(f) for f in files] if infos is None else list(infos)
+        batch = PcmBatch(files, infos, self.device, names)
+        B = len(batch)
+        ld = int(batch.lengths.max()) if ld is None and B else int(ld or 0)
+        out = torch.empty(B, ld, dtype=torch.float32, device=self.device)
+        status = torch.empty(B, dtype=torch.int32, device=self.device)
+        self.decode_pcm_into(batch, out, ld, status)
+        if check:
+            check_status(status.cpu().numpy(), batch.names)
+        return out, status
+
+    def decode_pcm_into(self, batch, out, ld, status, stream=None):
+        """vp_pcm_decode of a pcm.PcmBatch into ``out``, contiguous CUDA float32 holding B rows of ``ld`` (a matrix or a
+        flat staging slot), and the int32 ``status`` on ``stream`` (default: the current stream)."""
+        B = len(batch)
+        if B == 0:
+            return
+        assert out.dtype == torch.float32 and out.is_cuda and out.is_contiguous() and out.numel() >= B * ld
+        assert status.dtype == torch.int32 and status.is_cuda and status.numel() >= B
+        stream = torch.cuda.current_stream(self.device) if stream is None else stream
+        _check(self._h, L.lib().vp_pcm_decode(
+            self._h, C.c_void_p(batch.data.data_ptr()), batch.nbytes, C.c_void_p(batch.info.data_ptr()), B,
+            C.c_void_p(out.data_ptr()), int(ld), C.c_void_p(status.data_ptr()), C.c_void_p(stream.cuda_stream)))
+
     # ---- verification metrics (csrc/verify.cu) ----
     def verify(self, scores, labels=None, trial_labels=None, enroll_labels=None, p_target=0.01, c_miss=1, c_fa=1,
                sorted_out=False):

@@ -25,7 +25,7 @@ import torch
 import yaml
 from loguru import logger
 
-from .audio import AudioSegment, FlacSegment, decode_segments, device_samples
+from .audio import AudioSegment, FlacSegment, PcmSegment, decode_segments, device_samples
 from .data_utils.featurizer import AudioFeaturizer
 from .engine import Engine
 from .infer_utils.speaker_diarization import SpeakerDiarization
@@ -302,7 +302,8 @@ class MVectorPredictor:
 
     def _embed_waves(self, waves, lmax, masked, to_numpy=True, group=None, rates=None):
         """waves: list of 1-D float32 arrays, decoded, at ``rates`` Hz (None: all at the model's rate), or a device-rows
-        object (DeviceWindows, flac.DeviceFlacRows: ``lens``, ``gather``, ``check``, rows written on the device)
+        object (DeviceWindows, flac.DeviceFlacRows, pcm.DevicePcmRows: ``lens``, ``gather``, ``check``, rows written on
+        the device)
         -> [B, embd_dim] (np.float32, or the device tensor with ``to_numpy=False``).
         ``lmax`` is the longest item AFTER resampling.
 
@@ -322,8 +323,8 @@ class MVectorPredictor:
         event of their stage's copies and write straight into the [B, T, F] feature buffer; as soon as the features of a
         backbone chunk (``_host_chunks``) are complete the main stream runs its program, under the next stage's gather and
         copies.  With device rows a stage's rows are written into its device slot on the copy stream instead -- by
-        vp_gather_windows (DeviceWindows) or vp_flac_decode (DeviceFlacRows) -- and everything after that is the same.
-        One D2H of the result at the end; a refused FLAC stream raises ValueError after it."""
+        vp_gather_windows (DeviceWindows), vp_flac_decode (DeviceFlacRows) or vp_pcm_decode (DevicePcmRows) -- and
+        everything after that is the same.  One D2H of the result at the end; a refused row raises ValueError after it."""
         from . import _lib as L
         import ctypes as C
         import time
@@ -345,7 +346,7 @@ class MVectorPredictor:
         lib = L.lib()
         F = fz.feature_dim
         ds_conf = self.configs.dataset_conf.dataset
-        dev_rows = hasattr(waves, 'gather')              # DeviceWindows / DeviceFlacRows: rows written on the device
+        dev_rows = hasattr(waves, 'gather')              # DeviceWindows / DeviceFlacRows / DevicePcmRows
         lens = np.asarray(waves.lens, dtype=np.int32) if dev_rows else np.fromiter(map(len, waves), dtype=np.int32, count=B)
         plan = None
         gain_db = ds_conf.target_dB if ds_conf.use_dB_normalization else None
@@ -448,7 +449,7 @@ class MVectorPredictor:
         mark('all kernels enqueued')
         out = emb.cpu().numpy() if to_numpy else emb
         if dev_rows:
-            waves.check()                               # a refused FLAC stream: after the result copy
+            waves.check()                               # a refused FLAC stream or PCM row: after the result copy
         if flags is not None:
             plan.check(flags.cpu().numpy(), waves)      # after the result copy: no extra synchronise
         mark('result on host' if to_numpy else 'returned device tensor')
@@ -493,7 +494,7 @@ class MVectorPredictor:
     def predict(self, audio_data, sample_rate=16000):
         """预测一个音频的特征 (predict.py:214-229) -> np.ndarray [embd_dim]"""
         seg = self._load_audio(audio_data=audio_data, sample_rate=sample_rate)
-        waves = self._flac_rows([seg]) or [np.ascontiguousarray(seg.samples, dtype=np.float32)]
+        waves = self._device_rows([seg]) or [np.ascontiguousarray(seg.samples, dtype=np.float32)]
         lmax = int(self._output_lengths(self._row_lengths(waves), [seg.sample_rate])[0])
         return self._embed_waves(waves, lmax, masked=False, rates=[seg.sample_rate])[0]
 
@@ -521,19 +522,22 @@ class MVectorPredictor:
             if len(audios_data) == 0 or shortest / float(sample_rate) >= ds.min_duration:
                 return list(audios_data), [int(sample_rate)] * len(audios_data)
         segs = [self._load_audio(audio_data=a, sample_rate=sample_rate) for a in audios_data]
-        rows = self._flac_rows(segs)
+        rows = self._device_rows(segs)
         if rows is not None:
             return rows, [s.sample_rate for s in segs]
         decode_segments(segs, self._audio_featurizer.engine)   # a mixed list: its FLAC items in one device decode
         return [np.ascontiguousarray(s.samples, dtype=np.float32) for s in segs], [s.sample_rate for s in segs]
 
-    def _flac_rows(self, segs):
-        """DeviceFlacRows of ``segs`` when every one is an undecoded FLAC segment (their compressed bytes go up in one
-        pinned copy on the copy stream and each stage decodes into its slot), else None."""
-        if not segs or not all(isinstance(s, FlacSegment) and s._samples is None for s in segs):
-            return None
+    def _device_rows(self, segs):
+        """flac.DeviceFlacRows of ``segs`` when every one is an undecoded FLAC segment, pcm.DevicePcmRows when every one
+        is an undecoded PCM container segment (the files' bytes go up in one pinned copy on the copy stream and each
+        stage decodes into its slot), else None: a mixed list is staged from the host."""
         from .flac import DeviceFlacRows
-        return DeviceFlacRows(self._audio_featurizer.engine, segs, self._staging_stream())
+        from .pcm import DevicePcmRows
+        for seg_type, rows_type in ((FlacSegment, DeviceFlacRows), (PcmSegment, DevicePcmRows)):
+            if segs and all(isinstance(s, seg_type) and s._samples is None for s in segs):
+                return rows_type(self._audio_featurizer.engine, segs, self._staging_stream())
+        return None
 
     @staticmethod
     def _row_lengths(waves):
