@@ -3,12 +3,14 @@
 ``resample``, ``normalize``, ``vad``.  yeaudio (requirements.txt:12) is a third-party package absent from the reference tree and
 from this image; decoding/resampling sit OUTSIDE the parity boundary (SURVEY.md 8a3: parity starts at identical
 waveforms).  Decoding covers the uncompressed PCM containers -- WAV (integer, float, A-law and mu-law, also
-WAVE_FORMAT_EXTENSIBLE), RF64 / BW64 and AIFF / AIFF-C -- and native FLAC (RFC 9639).  Either segment knows its rate and
-duration from the header alone.  A FLAC segment is decoded by vp_flac_decode the first time its samples are read; a PCM
-segment's samples are converted by numpy on first read (pcm.to_mono), and both give a device row without a host copy
-(``decode_device``: vp_flac_decode / vp_pcm_decode).  Integers become float32 mono with ``pcm_to_mono``; pcm.py states
-the rule for floats and G.711.  Other input, and a RIFF file the PCM parser refuses, still goes to the standard
-library's ``wave`` reader."""
+WAVE_FORMAT_EXTENSIBLE), RF64 / BW64 and AIFF / AIFF-C -- and native FLAC (RFC 9639).  Both are EncodedSegments: a
+file kept as its bytes, whose rate and duration come from the header alone.  A FLAC segment is decoded by vp_flac_decode
+the first time its samples are read; a PCM segment's samples are converted by numpy on first read (pcm.to_mono), and
+both give a device row without a host copy (``decode_device``).  On the device an encoded file goes through one path
+whatever its codec: an EncodedBatch uploads the files' bytes in one pinned copy, the codec's subclass (flac.FlacBatch,
+pcm.PcmBatch) adds its tables and its decode, and DeviceEncodedRows writes the staging rows of ``_embed_waves`` from it.
+Integers become float32 mono with ``pcm_to_mono``; pcm.py states the rule for floats and G.711.  Other input, and a
+RIFF file the PCM parser refuses, still goes to the standard library's ``wave`` reader."""
 import io
 import os
 import wave
@@ -74,7 +76,7 @@ def device_samples(seg, engine):
     """A segment's samples as a CUDA float32 row on ``engine``'s device: an undecoded FLAC or PCM segment is converted
     there from its file's bytes and its samples never visit the host; any other segment's samples are uploaded."""
     import torch
-    if isinstance(seg, (FlacSegment, PcmSegment)) and seg._samples is None:
+    if isinstance(seg, EncodedSegment) and seg._samples is None:
         return seg.decode_device(engine)
     return torch.from_numpy(np.ascontiguousarray(seg.samples, dtype=np.float32)).to(engine.device)
 
@@ -241,81 +243,138 @@ class AudioSegment:
         return out
 
 
-class FlacSegment(AudioSegment):
-    """A native FLAC stream: ``sample_rate`` and ``duration`` come from STREAMINFO without decoding; ``samples`` are
-    decoded on the current CUDA device (vp_flac_decode) the first time they are read, and ``decode_device`` gives them
-    as a device row without a host copy.  ``name`` labels the stream in errors."""
+class EncodedSegment(AudioSegment):
+    """An encoded audio file kept as its bytes: ``sample_rate`` and ``duration`` come from the header (``info``) without
+    decoding; ``samples`` are converted on the host the first time they are read (``_convert``), and ``decode_device``
+    gives them as a device row without a host copy.  ``name`` labels the file in errors.  A subclass names its header
+    parser, its host conversion and its ``batch_type`` (an EncodedBatch subclass holding the codec's device decode)."""
+
+    def __init__(self, data, name, parse, batch_type):
+        self.data = bytes(data)
+        self.info = parse(self.data)
+        self.name = str(name)
+        self.batch_type = batch_type
+        self.sample_rate = self.info.sample_rate
+        self._samples = None
+
+    @property
+    def samples(self):
+        if self._samples is None:
+            self._samples = self._convert()
+        return self._samples
+
+    @samples.setter
+    def samples(self, value):
+        self._samples = value
+
+    @property
+    def duration(self):
+        if self._samples is None:
+            return self.info.duration
+        return self._samples.shape[0] / float(self.sample_rate)
+
+    def decode_device(self, engine):
+        """The decoded file as a CUDA float32 row on ``engine``'s device (ValueError when refused); the row is kept, so
+        a second call on the same device decodes nothing."""
+        row = getattr(self, '_device_row', None)
+        if row is None or row.device != engine.device:
+            rows, _ = engine.decode_batch(self.batch_type([self.data], [self.info], engine.device, [self.name]))
+            self._device_row = row = rows[0]
+        return row
+
+
+class FlacSegment(EncodedSegment):
+    """A native FLAC stream (``info``: its flac.StreamInfo).  There is no host decoder: ``samples`` are decoded on the
+    current CUDA device (vp_flac_decode) by ``decode_segments``."""
 
     def __init__(self, data, name='<flac>'):
-        from .flac import parse_streaminfo
-        self.data = bytes(data)
-        self.info = parse_streaminfo(self.data)
-        self.name = str(name)
-        self.sample_rate = self.info.sample_rate
-        self._samples = None
+        from .flac import FlacBatch, parse_streaminfo
+        super().__init__(data, name, parse_streaminfo, FlacBatch)
 
-    @property
-    def samples(self):
-        if self._samples is None:
-            decode_segments([self])
+    def _convert(self):
+        decode_segments([self])
         return self._samples
 
-    @samples.setter
-    def samples(self, value):
-        self._samples = value
 
-    @property
-    def duration(self):
-        if self._samples is None:
-            return self.info.duration
-        return self._samples.shape[0] / float(self.sample_rate)
-
-    def decode_device(self, engine):
-        """The decoded stream as a CUDA float32 row [total_samples] on ``engine``'s device (ValueError when refused);
-        the row is kept, so a second call on the same device decodes nothing."""
-        row = getattr(self, '_device_row', None)
-        if row is None or row.device != engine.device:
-            rows, _ = engine.decode_flac([self.data], [self.info], [self.name])
-            self._device_row = row = rows[0]
-        return row
-
-
-class PcmSegment(AudioSegment):
-    """An uncompressed PCM container file (WAV, RF64 / BW64, AIFF / AIFF-C): ``sample_rate`` and ``duration`` come from
-    the header without converting; ``samples`` are converted on the host by numpy (pcm.to_mono) the first time they are
-    read, and ``decode_device`` converts the file's bytes on the device (vp_pcm_decode) into the same row.  ``name``
-    labels the file in errors."""
+class PcmSegment(EncodedSegment):
+    """An uncompressed PCM container file (WAV, RF64 / BW64, AIFF / AIFF-C; ``info``: its pcm.PcmInfo): ``samples`` are
+    converted on the host by numpy (pcm.to_mono), the same row vp_pcm_decode gives on the device."""
 
     def __init__(self, data, name='<pcm>'):
-        from .pcm import parse_header
-        self.data = bytes(data)
-        self.info = parse_header(self.data)
-        self.name = str(name)
-        self.sample_rate = self.info.sample_rate
-        self._samples = None
+        from .pcm import PcmBatch, parse_header
+        super().__init__(data, name, parse_header, PcmBatch)
 
-    @property
-    def samples(self):
-        if self._samples is None:
-            from .pcm import to_mono
-            self._samples = to_mono(self.data, self.info)
-        return self._samples
+    def _convert(self):
+        from .pcm import to_mono
+        return to_mono(self.data, self.info)
 
-    @samples.setter
-    def samples(self, value):
-        self._samples = value
 
-    @property
-    def duration(self):
-        if self._samples is None:
-            return self.info.duration
-        return self._samples.shape[0] / float(self.sample_rate)
+class EncodedBatch:
+    """Device inputs of one decode over several encoded files: their bytes concatenated in ``data`` (file i from
+    ``offsets[i]``, ``nbytes`` in all) and each file's decoded length in ``lengths``.  ``names`` label the items in errors.
+    A subclass adds its codec's per-row tables (``_tables``), the batch of rows lo..hi a stage decodes
+    (``rows(lo, hi, stream)``), the engine's decode (``decode_into``), a row decoded for the host (``host_row``), and the
+    ``label`` and ``unit`` its errors name."""
 
-    def decode_device(self, engine):
-        """The converted file as a CUDA float32 row [frames] on ``engine``'s device; the row is kept, so a second call on
-        the same device converts nothing."""
-        row = getattr(self, '_device_row', None)
-        if row is None or row.device != engine.device:
-            rows, _ = engine.decode_pcm([self.data], [self.info], [self.name])
-            self._device_row = row = rows[0]
-        return row
+    def __init__(self, files, infos, device, names=None, stream=None):
+        """The bytes go up in one pinned copy, then the tables, on ``stream`` (default: the current stream)."""
+        import torch
+        self.infos = list(infos)
+        self.names = list(names) if names is not None else [f'item {i}' for i in range(len(self.infos))]
+        self.lengths = np.array([self._length(si) for si in self.infos], dtype=np.int64)
+        sizes = np.array([len(f) for f in files], dtype=np.int64)
+        self.offsets = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
+        self.nbytes = int(self.offsets[-1])
+        with torch.cuda.stream(stream):
+            host = torch.empty(max(self.nbytes, 1), dtype=torch.uint8, pin_memory=True)
+            hv = host.numpy()
+            for o, f in zip(self.offsets[:-1], files):
+                hv[o:o + len(f)] = np.frombuffer(f, dtype=np.uint8)
+            self.data = host.to(device, non_blocking=True)
+            self._tables(device)
+        self._host = host            # the pinned source stays alive until the copy has run
+
+    def __len__(self):
+        return len(self.infos)
+
+    def file(self, i):
+        """The bytes of file i, read back from the pinned source."""
+        return bytes(self._host.numpy()[self.offsets[i]:self.offsets[i + 1]])
+
+
+def check_status(status, names, label, unit):
+    """Raise ValueError naming every refused item of a ``label`` decode (status: host int32 array, one per ``unit``)."""
+    bad = np.flatnonzero(np.asarray(status))
+    if bad.size:
+        items = ', '.join(f'{names[i]} (status {int(status[i])})' for i in bad[:8])
+        raise ValueError(f'{label} decode refused {bad.size} {unit}(s): {items}')
+
+
+class DeviceEncodedRows:
+    """Rows of ``_embed_waves`` decoded on the device from EncodedSegments of one class: row i is file i at its native
+    rate, ``lens[i]`` samples zero filled to the slot's width.  The files' bytes go up in one pinned copy on the copy
+    stream; a staging slot is then written by the device decode of its rows instead of the host gather and H2D copy.
+    ``check`` raises ValueError naming a refused file (after the caller's result copy)."""
+
+    def __init__(self, engine, segs, copy_stream):
+        import torch
+        self.engine, self.stream = engine, copy_stream
+        self.batch = segs[0].batch_type([s.data for s in segs], [s.info for s in segs], engine.device,
+                                        [s.name for s in segs], copy_stream)
+        self.lens = np.array(self.batch.lengths.tolist(), dtype=np.int32)    # a length past int32 raises, never wraps
+        with torch.cuda.stream(copy_stream):
+            self.status = torch.zeros(len(segs), dtype=torch.int32, device=engine.device)
+
+    def __len__(self):
+        return len(self.batch)
+
+    def gather(self, lo, hi, dst, ld, stream):
+        """Rows lo..hi decoded into the device slot ``dst`` [hi - lo, ld] on ``stream``."""
+        self.batch.rows(lo, hi, self.stream).decode_into(self.engine, dst, ld, self.status[lo:hi], stream)
+
+    def __getitem__(self, i):
+        """Host copy of row i (ConditionPlan.check recomputes a flagged row's gain from it)."""
+        return self.batch.host_row(i, self.engine)
+
+    def check(self):
+        check_status(self.status.cpu().numpy(), self.batch.names, self.batch.label, self.batch.unit)

@@ -194,17 +194,9 @@ class Engine:
         vp_flac_decode, every row mixed to mono exactly as audio.pcm_to_mono mixes the same integers.  ``ld`` defaults to
         the longest stream.  With ``check`` a non-zero status raises ValueError naming the item (``names``, default
         'item i'); that waits for the decode."""
-        from .flac import FlacBatch, check_status, parse_streaminfo
-        infos = [parse_streaminfo(s) for s in streams] if infos is None else list(infos)
-        batch = FlacBatch(streams, infos, self.device, names)
-        B = len(batch)
-        ld = int(batch.lengths.max()) if ld is None and B else int(ld or 0)
-        out = torch.empty(B, ld, dtype=torch.float32, device=self.device)
-        status = torch.empty(B, dtype=torch.int32, device=self.device)
-        self.decode_flac_into(batch, out, ld, status)
-        if check:
-            check_status(status.cpu().numpy(), batch.names)
-        return out, status
+        from .flac import FlacBatch, parse_streaminfo
+        infos = [parse_streaminfo(s) for s in streams] if infos is None else infos
+        return self.decode_batch(FlacBatch(streams, infos, self.device, names), ld, check)
 
     def decode_flac_into(self, batch, out, ld, status, stream=None):
         """vp_flac_decode of a flac.FlacBatch into ``out``, contiguous CUDA float32 holding B rows of ``ld`` (a matrix or a
@@ -232,17 +224,9 @@ class Engine:
         vp_pcm_decode, every row bit-identical to pcm.to_mono.  ``ld`` defaults to the longest file.  With ``check`` a
         non-zero status raises ValueError naming the item (``names``, default 'item i'); that waits for the
         conversion."""
-        from .pcm import PcmBatch, check_status, parse_header
-        infos = [parse_header(f) for f in files] if infos is None else list(infos)
-        batch = PcmBatch(files, infos, self.device, names)
-        B = len(batch)
-        ld = int(batch.lengths.max()) if ld is None and B else int(ld or 0)
-        out = torch.empty(B, ld, dtype=torch.float32, device=self.device)
-        status = torch.empty(B, dtype=torch.int32, device=self.device)
-        self.decode_pcm_into(batch, out, ld, status)
-        if check:
-            check_status(status.cpu().numpy(), batch.names)
-        return out, status
+        from .pcm import PcmBatch, parse_header
+        infos = [parse_header(f) for f in files] if infos is None else infos
+        return self.decode_batch(PcmBatch(files, infos, self.device, names), ld, check)
 
     def decode_pcm_into(self, batch, out, ld, status, stream=None):
         """vp_pcm_decode of a pcm.PcmBatch into ``out``, contiguous CUDA float32 holding B rows of ``ld`` (a matrix or a
@@ -256,6 +240,20 @@ class Engine:
         _check(self._h, L.lib().vp_pcm_decode(
             self._h, C.c_void_p(batch.data.data_ptr()), batch.nbytes, C.c_void_p(batch.info.data_ptr()), B,
             C.c_void_p(out.data_ptr()), int(ld), C.c_void_p(status.data_ptr()), C.c_void_p(stream.cuda_stream)))
+
+    def decode_batch(self, batch, ld=None, check=True):
+        """An audio.EncodedBatch (flac.FlacBatch, pcm.PcmBatch) decoded by its codec's kernel -> (rows CUDA float32
+        [B, ld] at the native rates, zero filled past each item's length, status CUDA int32 [B]); ``ld`` defaults to the
+        longest item.  With ``check`` a non-zero status raises ValueError naming the item; that waits for the decode."""
+        from .audio import check_status
+        B = len(batch)
+        ld = int(batch.lengths.max()) if ld is None and B else int(ld or 0)
+        out = torch.empty(B, ld, dtype=torch.float32, device=self.device)
+        status = torch.empty(B, dtype=torch.int32, device=self.device)
+        batch.decode_into(self, out, ld, status)
+        if check:
+            check_status(status.cpu().numpy(), batch.names, batch.label, batch.unit)
+        return out, status
 
     # ---- verification metrics (csrc/verify.cu) ----
     def verify(self, scores, labels=None, trial_labels=None, enroll_labels=None, p_target=0.01, c_miss=1, c_fa=1,

@@ -2,10 +2,13 @@
 
 The host reads only the ``fLaC`` magic and the metadata blocks -- STREAMINFO gives the rate, channel count, bit depth
 and length, so a segment's duration is known without decoding.  The frames are decoded on the device by
-``vp_flac_decode`` (csrc/flac.cu); there is no host decoder behind it."""
+``vp_flac_decode`` (csrc/flac.cu); there is no host decoder behind it.  ``FlacBatch`` is the codec's audio.EncodedBatch:
+the per-stream tables vp_flac_decode reads and the rebased batch of a staging stage's rows."""
 from dataclasses import dataclass
 
 import numpy as np
+
+from .audio import EncodedBatch
 
 MAGIC = b'fLaC'
 
@@ -95,94 +98,46 @@ def _info_struct(si):
                     si.min_framesize, si.max_framesize, 0)
 
 
-class FlacBatch:
-    """Device inputs of one vp_flac_decode over several streams: the concatenated bytes and the per-stream tables.
-    ``names`` label the items in errors."""
+class FlacBatch(EncodedBatch):
+    """Device inputs of one vp_flac_decode over several streams: the concatenated bytes and the per-stream tables
+    (``offsets`` and ``frame_off`` as vp_flac_decode's stream and first-frame offsets, a vp_flac_info per stream)."""
+    label, unit = 'FLAC', 'stream'
 
-    def __init__(self, streams, infos, device, names=None, stream=None):
-        """The bytes go up in one pinned copy on ``stream`` (default: the current stream)."""
+    @staticmethod
+    def _length(si):
+        return si.total_samples
+
+    def _tables(self, device):
         import torch
-        if stream is not None:
-            with torch.cuda.stream(stream):
-                self.__init__(streams, infos, device, names)
-            return
-        self.infos = list(infos)
-        self.names = list(names) if names is not None else [f'item {i}' for i in range(len(self.infos))]
-        sizes = np.array([len(s) for s in streams], dtype=np.int64)
-        self.stream_off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-        self.frame_off = self.stream_off[:-1] + np.array([si.frame_offset for si in self.infos], dtype=np.int64)
-        self.nbytes = int(self.stream_off[-1])
+        self.frame_off = self.offsets[:-1] + np.array([si.frame_offset for si in self.infos], dtype=np.int64)
         self.max_frames = int(sum(-(-si.total_samples // si.min_blocksize) for si in self.infos))
-        self.lengths = np.array([si.total_samples for si in self.infos], dtype=np.int64)
-        host = torch.empty(max(self.nbytes, 1), dtype=torch.uint8, pin_memory=True)
-        hv = host.numpy()
-        for o, s in zip(self.stream_off[:-1], streams):
-            hv[o:o + len(s)] = np.frombuffer(s, dtype=np.uint8)
-        self.data = host.to(device, non_blocking=True)
         raw = b''.join(bytes(_info_struct(si)) for si in self.infos)
         self.info = torch.frombuffer(bytearray(raw or b'\0'), dtype=torch.uint8).to(device)
-        self.stream_off_dev = torch.from_numpy(self.stream_off).to(device)
+        self.stream_off_dev = torch.from_numpy(self.offsets).to(device)
         self.frame_off_dev = torch.from_numpy(self.frame_off).to(device)
-        self._host = host            # the pinned source stays alive until the copy has run
-        self._src = [memoryview(hv[o:o + len(s)]) for o, s in zip(self.stream_off[:-1], streams)]
 
-    def __len__(self):
-        return len(self.infos)
-
-
-def check_status(status, names):
-    """Raise ValueError naming every refused item of a decode (status: host int32 array)."""
-    bad = np.flatnonzero(np.asarray(status))
-    if bad.size:
-        items = ', '.join(f'{names[i]} (status {int(status[i])})' for i in bad[:8])
-        raise ValueError(f'FLAC decode refused {bad.size} stream(s): {items}')
-
-
-class DeviceFlacRows:
-    """Rows of ``_embed_waves`` decoded from FLAC streams on the device: row i is stream i at its native rate, ``lens[i]``
-    samples zero filled to the slot's width.  The compressed bytes of every row go up in one pinned copy on the copy
-    stream; a staging slot is then written by vp_flac_decode of its rows instead of the host gather and H2D copy.
-    ``check`` raises ValueError naming a refused stream (after the caller's result copy)."""
-
-    def __init__(self, engine, segs, copy_stream):
+    def rows(self, lo, hi, stream):
+        """The batch of rows lo..hi: the bytes stay where they are, the tables are rebased onto row lo and uploaded on
+        ``stream``.  The scan and link passes walk every byte from ``data`` on, so a stage passes only its own bytes."""
         import torch
-        self.engine, self.stream = engine, copy_stream
-        self.infos = [s.info for s in segs]
-        self.names = [s.name for s in segs]
-        self.lens = np.array([si.total_samples for si in self.infos], dtype=np.int32)
-        self.batch = FlacBatch([s.data for s in segs], self.infos, engine.device, self.names, stream=copy_stream)
-        with torch.cuda.stream(copy_stream):
-            self.status = torch.zeros(len(segs), dtype=torch.int32, device=engine.device)
-
-    def __len__(self):
-        return len(self.infos)
-
-    def _stage(self, lo, hi):
-        """A FlacBatch view of rows lo..hi: the bytes stay where they are, the tables are rebased onto row lo."""
-        import torch
-        b = self.batch
         v = FlacBatch.__new__(FlacBatch)
-        base = int(b.stream_off[lo])
-        v.infos, v.names = b.infos[lo:hi], b.names[lo:hi]
-        v.stream_off, v.frame_off = b.stream_off[lo:hi + 1] - base, b.frame_off[lo:hi] - base
-        v.nbytes = int(v.stream_off[-1])
+        base = int(self.offsets[lo])
+        v.infos, v.names = self.infos[lo:hi], self.names[lo:hi]
+        v.offsets, v.frame_off = self.offsets[lo:hi + 1] - base, self.frame_off[lo:hi] - base
+        v.nbytes = int(v.offsets[-1])
         v.max_frames = int(sum(-(-si.total_samples // si.min_blocksize) for si in v.infos))
-        v.lengths = b.lengths[lo:hi]
-        v.data = b.data[base:]
-        v.info = b.info[lo * (b.info.numel() // len(b)):]
-        with torch.cuda.stream(self.stream):
-            v.stream_off_dev = torch.from_numpy(v.stream_off).to(self.engine.device, non_blocking=True)
-            v.frame_off_dev = torch.from_numpy(v.frame_off).to(self.engine.device, non_blocking=True)
+        v.lengths = self.lengths[lo:hi]
+        v.data = self.data[base:]
+        v.info = self.info[lo * (self.info.numel() // len(self)):]
+        with torch.cuda.stream(stream):
+            v.stream_off_dev = torch.from_numpy(v.offsets).to(self.data.device, non_blocking=True)
+            v.frame_off_dev = torch.from_numpy(v.frame_off).to(self.data.device, non_blocking=True)
         return v
 
-    def gather(self, lo, hi, dst, ld, stream):
-        """Rows lo..hi decoded into the device slot ``dst`` [hi - lo, ld] on ``stream``."""
-        self.engine.decode_flac_into(self._stage(lo, hi), dst, ld, self.status[lo:hi], stream)
+    def decode_into(self, engine, out, ld, status, stream=None):
+        engine.decode_flac_into(self, out, ld, status, stream)
 
-    def __getitem__(self, i):
-        """Host copy of row i (ConditionPlan.check recomputes a flagged row's gain from it)."""
-        rows, _ = self.engine.decode_flac([bytes(self.batch._src[i])], [self.infos[i]], [self.names[i]])
+    def host_row(self, i, engine):
+        """Stream i decoded on ``engine``'s device and copied to the host."""
+        rows, _ = engine.decode_flac([self.file(i)], [self.infos[i]], [self.names[i]])
         return rows[0].cpu().numpy()
-
-    def check(self):
-        check_status(self.status.cpu().numpy(), self.names)

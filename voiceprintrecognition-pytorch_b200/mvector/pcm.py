@@ -7,11 +7,14 @@ parser reads only the headers -- never a sample -- so a segment knows its rate a
 samples become float32 mono by one rule (include/vpb200.h): integers of container width N as x / 2^(N-1)
 (``audio.pcm_to_mono``), float32 as stored, float64 rounded to float32, G.711 through its 16-bit expansion, then
 numpy's float32 mean over the channels.  ``to_mono`` applies it with numpy; ``vp_pcm_decode`` (csrc/pcm.cu) applies it
-on the device, bit for bit the same."""
+on the device, bit for bit the same, to a ``PcmBatch``: the codec's audio.EncodedBatch, whose per-row table holds each
+row's absolute byte offset."""
 import struct
 from dataclasses import dataclass
 
 import numpy as np
+
+from .audio import EncodedBatch
 
 # VP_PCM_* of include/vpb200.h
 U8, S8, S16LE, S16BE, S24LE, S24BE, S32LE, S32BE, F32LE, F32BE, F64LE, F64BE, ULAW, ALAW = range(1, 15)
@@ -276,37 +279,23 @@ def _info_struct(info, base):
     return CInfo(base + info.data_offset, info.frames, info.channels, info.format, 0, 0)
 
 
-class PcmBatch:
-    """Device inputs of one vp_pcm_decode over several files: their concatenated bytes and a vp_pcm_info per row.
-    ``names`` label the items in errors; ``rows(lo, hi)`` is the batch of rows lo..hi over the same bytes."""
+class PcmBatch(EncodedBatch):
+    """Device inputs of one vp_pcm_decode over several files: their concatenated bytes and a vp_pcm_info per row, which
+    holds the row's absolute byte offset, so ``rows(lo, hi)`` is a batch over the same bytes that uploads nothing."""
+    label, unit = 'PCM', 'row'
 
-    def __init__(self, files, infos, device, names=None, stream=None):
-        """The bytes go up in one pinned copy on ``stream`` (default: the current stream)."""
+    @staticmethod
+    def _length(si):
+        return si.frames
+
+    def _tables(self, device):
         import torch
-        if stream is not None:
-            with torch.cuda.stream(stream):
-                self.__init__(files, infos, device, names)
-            return
-        self.infos = list(infos)
-        self.names = list(names) if names is not None else [f'item {i}' for i in range(len(self.infos))]
-        sizes = np.array([len(f) for f in files], dtype=np.int64)
-        off = np.concatenate([[0], np.cumsum(sizes)]).astype(np.int64)
-        self.nbytes = int(off[-1])
-        self.lengths = np.array([si.frames for si in self.infos], dtype=np.int64)
-        host = torch.empty(max(self.nbytes, 1), dtype=torch.uint8, pin_memory=True)
-        hv = host.numpy()
-        for o, f in zip(off[:-1], files):
-            hv[o:o + len(f)] = np.frombuffer(f, dtype=np.uint8)
-        self.data = host.to(device, non_blocking=True)
-        raw = b''.join(bytes(_info_struct(si, int(o))) for si, o in zip(self.infos, off[:-1]))
+        raw = b''.join(bytes(_info_struct(si, int(o))) for si, o in zip(self.infos, self.offsets[:-1]))
         self.info = torch.frombuffer(bytearray(raw or b'\0'), dtype=torch.uint8).pin_memory().to(device,
                                                                                                  non_blocking=True)
-        self._host = host            # the pinned source stays alive until the copy has run
 
-    def __len__(self):
-        return len(self.infos)
-
-    def rows(self, lo, hi):
+    def rows(self, lo, hi, stream=None):
+        """The batch of rows lo..hi: a slice of the info table over the same bytes (``stream`` is unused)."""
         v = PcmBatch.__new__(PcmBatch)
         v.infos, v.names, v.nbytes, v.lengths, v.data = self.infos[lo:hi], self.names[lo:hi], self.nbytes, \
             self.lengths[lo:hi], self.data
@@ -314,42 +303,9 @@ class PcmBatch:
         v.info = self.info[lo * size:hi * size]
         return v
 
+    def decode_into(self, engine, out, ld, status, stream=None):
+        engine.decode_pcm_into(self, out, ld, status, stream)
 
-def check_status(status, names):
-    """Raise ValueError naming every refused row of a vp_pcm_decode (status: host int32 array)."""
-    bad = np.flatnonzero(np.asarray(status))
-    if bad.size:
-        items = ', '.join(f'{names[i]} (status {int(status[i])})' for i in bad[:8])
-        raise ValueError(f'PCM decode refused {bad.size} row(s): {items}')
-
-
-class DevicePcmRows:
-    """Rows of ``_embed_waves`` converted from PCM container files on the device: row i is file i at its native rate,
-    ``lens[i]`` samples zero filled to the slot's width.  The files' bytes go up in one pinned copy on the copy stream;
-    a staging slot is then written by vp_pcm_decode of its rows instead of the host gather and H2D copy.  The protocol
-    of flac.DeviceFlacRows: ``lens``, ``gather``, ``check``, ``__getitem__``."""
-
-    def __init__(self, engine, segs, copy_stream):
-        import torch
-        self.engine = engine
-        self.infos = [s.info for s in segs]
-        self.names = [s.name for s in segs]
-        self._data = [s.data for s in segs]
-        self.lens = np.array([si.frames for si in self.infos], dtype=np.int32)
-        self.batch = PcmBatch(self._data, self.infos, engine.device, self.names, stream=copy_stream)
-        with torch.cuda.stream(copy_stream):
-            self.status = torch.zeros(len(segs), dtype=torch.int32, device=engine.device)
-
-    def __len__(self):
-        return len(self.infos)
-
-    def gather(self, lo, hi, dst, ld, stream):
-        """Rows lo..hi converted into the device slot ``dst`` [hi - lo, ld] on ``stream``."""
-        self.engine.decode_pcm_into(self.batch.rows(lo, hi), dst, ld, self.status[lo:hi], stream)
-
-    def __getitem__(self, i):
-        """Host copy of row i (ConditionPlan.check recomputes a flagged row's gain from it): the same row by numpy."""
-        return to_mono(self._data[i], self.infos[i])
-
-    def check(self):
-        check_status(self.status.cpu().numpy(), self.names)
+    def host_row(self, i, engine):
+        """Row i converted by numpy: the same row as the device's."""
+        return to_mono(self.file(i), self.infos[i])

@@ -25,7 +25,7 @@ import torch
 import yaml
 from loguru import logger
 
-from .audio import AudioSegment, FlacSegment, PcmSegment, decode_segments, device_samples
+from .audio import AudioSegment, DeviceEncodedRows, EncodedSegment, decode_segments, device_samples
 from .data_utils.featurizer import AudioFeaturizer
 from .engine import Engine
 from .infer_utils.speaker_diarization import SpeakerDiarization
@@ -302,8 +302,7 @@ class MVectorPredictor:
 
     def _embed_waves(self, waves, lmax, masked, to_numpy=True, group=None, rates=None):
         """waves: list of 1-D float32 arrays, decoded, at ``rates`` Hz (None: all at the model's rate), or a device-rows
-        object (DeviceWindows, flac.DeviceFlacRows, pcm.DevicePcmRows: ``lens``, ``gather``, ``check``, rows written on
-        the device)
+        object (DeviceWindows, audio.DeviceEncodedRows: ``lens``, ``gather``, ``check``, rows written on the device)
         -> [B, embd_dim] (np.float32, or the device tensor with ``to_numpy=False``).
         ``lmax`` is the longest item AFTER resampling.
 
@@ -323,7 +322,7 @@ class MVectorPredictor:
         event of their stage's copies and write straight into the [B, T, F] feature buffer; as soon as the features of a
         backbone chunk (``_host_chunks``) are complete the main stream runs its program, under the next stage's gather and
         copies.  With device rows a stage's rows are written into its device slot on the copy stream instead -- by
-        vp_gather_windows (DeviceWindows), vp_flac_decode (DeviceFlacRows) or vp_pcm_decode (DevicePcmRows) -- and
+        vp_gather_windows (DeviceWindows), or vp_flac_decode / vp_pcm_decode (DeviceEncodedRows) -- and
         everything after that is the same.  One D2H of the result at the end; a refused row raises ValueError after it."""
         from . import _lib as L
         import ctypes as C
@@ -346,7 +345,7 @@ class MVectorPredictor:
         lib = L.lib()
         F = fz.feature_dim
         ds_conf = self.configs.dataset_conf.dataset
-        dev_rows = hasattr(waves, 'gather')              # DeviceWindows / DeviceFlacRows / DevicePcmRows
+        dev_rows = hasattr(waves, 'gather')              # DeviceWindows / DeviceEncodedRows
         lens = np.asarray(waves.lens, dtype=np.int32) if dev_rows else np.fromiter(map(len, waves), dtype=np.int32, count=B)
         plan = None
         gain_db = ds_conf.target_dB if ds_conf.use_dB_normalization else None
@@ -529,14 +528,11 @@ class MVectorPredictor:
         return [np.ascontiguousarray(s.samples, dtype=np.float32) for s in segs], [s.sample_rate for s in segs]
 
     def _device_rows(self, segs):
-        """flac.DeviceFlacRows of ``segs`` when every one is an undecoded FLAC segment, pcm.DevicePcmRows when every one
-        is an undecoded PCM container segment (the files' bytes go up in one pinned copy on the copy stream and each
-        stage decodes into its slot), else None: a mixed list is staged from the host."""
-        from .flac import DeviceFlacRows
-        from .pcm import DevicePcmRows
-        for seg_type, rows_type in ((FlacSegment, DeviceFlacRows), (PcmSegment, DevicePcmRows)):
-            if segs and all(isinstance(s, seg_type) and s._samples is None for s in segs):
-                return rows_type(self._audio_featurizer.engine, segs, self._staging_stream())
+        """audio.DeviceEncodedRows of ``segs`` when every one is an undecoded EncodedSegment of the same class (all FLAC
+        or all PCM containers: the files' bytes go up in one pinned copy on the copy stream and each stage decodes into
+        its slot), else None: a mixed list is staged from the host."""
+        if segs and all(isinstance(s, EncodedSegment) and s._samples is None and type(s) is type(segs[0]) for s in segs):
+            return DeviceEncodedRows(self._audio_featurizer.engine, segs, self._staging_stream())
         return None
 
     @staticmethod
