@@ -124,6 +124,20 @@ int vp_melspec(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const i
 int vp_mfcc(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep_frames, float* feats,
             float* scratch, void* stream);
 
+/* The configured front-end (vp_fbank, vp_melspec or vp_mfcc, whichever vp_frontend_set chose) on a ragged batch, every
+ * row as if it were the whole call: the reference's eval / feature-extraction mode (reader.py:82-107), which featurizes
+ * each file alone and zero-pads the features to the batch's longest (collate_fn.py:5-24).
+ *   wave  [B, ld] device floats, row b holding lens[b] samples (lens: device int32 [B], each in [0, ld])
+ *   T     the frames of the longest row, vp_num_frames(max lens[b]); 1 <= T <= vp_num_frames(ld)
+ *   feats [B, T, F]: row b's first T_b = vp_num_frames(lens[b]) frames are exactly what a one-row call on its lens[b]
+ *         samples returns (framing at the row's own end, CMN over its own frames, MFCC's top_db clamp against its own
+ *         maximum); frames T_b .. T-1 are +0.0.  Nothing is written past T.
+ *   scratch: device floats, at least vp_frontend_scratch_floats(B, n) for n the longest row's lens (ld always does).
+ * ld must pass the call's length check above; a row whose length breaks it gives unspecified features but reads no
+ * sample outside its own first lens[b]. */
+int vp_features_each(vp_handle* h, const float* wave, int32_t B, int32_t ld, const int32_t* lens, int32_t T, float* feats,
+                     float* scratch, void* stream);
+
 /* vp_mfcc in two stages, for callers that split ONE reference call over several processes (utterance sharding,
  * SURVEY.md 8e): the top_db clamp of torchaudio's MFCC uses the maximum over the WHOLE call, so a sharded call computes
  *   vp_mfcc_mel    : mel dB values of its shard into `scratch`, their maximum into max_out[0] (device float),

@@ -210,14 +210,7 @@ int vp_frontend_set_options(vp_handle* h, const vp_frontend_options* o) {
 
 int32_t vp_num_frames(const vp_handle* h, int32_t n) {
   if (!h || !h->fe_set) return -1;
-  const int hop = h->fe.hop, mode = h->fe_opt.frame_mode;
-  if (h->fe.kind == 0) {
-    if (mode == VP_FRAME_KALDI_REFLECT) return (n + hop / 2) / hop;
-    return n < h->fe.win_length ? 0 : 1 + (n - h->fe.win_length) / hop;
-  }
-  const int64_t Lp = (int64_t)n + 2 * (int64_t)h->fe_opt.pad;
-  if (mode == VP_FRAME_STFT_NOCENTER) return Lp < h->fe.n_fft ? 0 : (int32_t)(1 + (Lp - h->fe.n_fft) / hop);
-  return (int32_t)(1 + Lp / hop);
+  return frontend_frames(h->fe.kind, h->fe_opt.frame_mode, h->fe.win_length, h->fe.n_fft, h->fe.hop, h->fe_opt.pad, n);
 }
 
 // The waveform lengths torch accepts for the configured framing (kaldi.py:141, torch.stft / F.pad): "" when L fits.
@@ -239,14 +232,18 @@ int32_t vp_feature_dim(const vp_handle* h) {
 
 static size_t round4(size_t n) { return (n + 3) & ~(size_t)3; }
 
-// scratch layout: [CMN partial sums B*nblk*F] and, for MFCC, [per-CTA maxima B*nblk] [dB mel values B*T*n_mels]
-size_t vp_frontend_scratch_floats(const vp_handle* h, int32_t B, int32_t Lpad) {
-  int T = vp_num_frames(h, Lpad);
-  if (T <= 0) return 0;
+// scratch layout of a call with T frames: [CMN partial sums B*nblk*F], for MFCC [per-CTA maxima B*nblk] [dB mel values
+// B*T*n_mels], then [the rows' frame counts: B int32] of a ragged call
+static size_t frontend_scratch_floats(const vp_handle* h, int B, int T) {
   size_t nblk = (T + FPB - 1) / FPB;
   size_t n = round4((size_t)B * nblk * vp_feature_dim(h));
   if (h->fe.post == 1) n += round4((size_t)B * nblk) + round4((size_t)B * T * h->fe.n_mels);
   return n;
+}
+size_t vp_frontend_scratch_floats(const vp_handle* h, int32_t B, int32_t Lpad) {
+  int T = vp_num_frames(h, Lpad);
+  if (T <= 0) return 0;
+  return frontend_scratch_floats(h, B, T) + round4((size_t)B);
 }
 
 // The waveform length check of every front-end call: "" when B rows of L samples give at least one frame.
@@ -258,10 +255,11 @@ static const char* frontend_call_error(const vp_handle* h, int B, int L) {
 }
 
 // The planned FrontendParams of a call on B rows of L samples (frontend_call_error(h, B, L) == ""), buffer pointers
-// left null: the one place the launch shape comes from, for run_frontend and vp_frontend_plan_info alike.
-static FrontendParams frontend_params(const vp_handle* h, int B, int L) {
+// left null: the one place the launch shape comes from, for run_frontend and vp_frontend_plan_info alike.  T: the
+// frames of the call, vp_num_frames(L) when < 0 (a ragged call passes its longest row's).
+static FrontendParams frontend_params(const vp_handle* h, int B, int L, int T = -1) {
   FrontendParams p{};
-  const int T = vp_num_frames(h, L);
+  if (T < 0) T = vp_num_frames(h, L);
   p.window = h->d_window; p.twiddle = h->d_twiddle;
   p.mel_start = h->d_mel_start; p.mel_count = h->d_mel_count; p.mel_off = h->d_mel_off; p.mel_w = h->d_mel_w;
   p.mel_nw = h->mel_nw;
@@ -279,8 +277,10 @@ static FrontendParams frontend_params(const vp_handle* h, int B, int L) {
 // want_kind / want_post: -1 = whatever is configured (vp_embed_wave).
 // stage: 0 = the whole front-end; 1 = MFCC mel stage only (maximum -> ext_max[0]); 2 = MFCC clamp/DCT/CMN only, clamping
 // against the externally reduced maximum ext_max[0].
+// lens (device int32 [B]) non-null: a ragged call of T frames, row b featurized alone on its first lens[b] samples.
 static int run_frontend(vp_handle* h, int want_kind, int want_post, const float* wave, int B, int L, const int32_t* keep,
-                        float* feats, float* scratch, cudaStream_t st, int stage = 0, float* ext_max = nullptr) {
+                        float* feats, float* scratch, cudaStream_t st, int stage = 0, float* ext_max = nullptr,
+                        const int32_t* lens = nullptr, int T_call = -1) {
   if (!h) return VP_ERR_INVALID;
   if (!h->fe_set) return fail(h, VP_ERR_INVALID, "front-end not configured (vp_frontend_set)");
   if (want_kind >= 0 && h->fe.kind != want_kind) return fail(h, VP_ERR_INVALID, "front-end kind mismatch");
@@ -289,10 +289,17 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
   if (stage != 0 && (h->fe.post != 1 || !ext_max)) return fail(h, VP_ERR_INVALID, "two-stage calls are for the MFCC front-end");
   const char* len_err = frontend_call_error(h, B, L);
   if (*len_err) return fail(h, VP_ERR_INVALID, "waveform of %d samples: %s", L, len_err);
+  if (lens && (T_call < 1 || T_call > vp_num_frames(h, L)))
+    return fail(h, VP_ERR_INVALID, "T = %d frames: need 1 <= T <= %d, the frames of a %d-sample row", T_call,
+                vp_num_frames(h, L), L);
   CUDA_TRY(h, cudaSetDevice(h->device));
-  FrontendParams p = frontend_params(h, B, L);
+  FrontendParams p = frontend_params(h, B, L, lens ? T_call : -1);
   p.wave = wave; p.feats = feats; p.partial = scratch;
   const int T = p.T;
+  if (lens) {
+    p.lens = lens;
+    p.row_T = reinterpret_cast<int*>(scratch + frontend_scratch_floats(h, B, T));
+  }
   if (h->fe.post == 1) {
     MfccParams m;
     float* cta_max = scratch + round4((size_t)B * p.nblk * h->fe.n_out);
@@ -301,6 +308,7 @@ static int run_frontend(vp_handle* h, int want_kind, int want_post, const float*
     m.mel = mel; m.cta_max = cta_max; m.dct = h->d_dct; m.feats = feats; m.partial = scratch;
     m.B = B; m.T = T; m.M = h->fe.n_mels; m.K = h->fe.n_out; m.fpb = FPB; m.nblk = p.nblk; m.n_max = B * p.nblk;
     m.top_db = h->fe.top_db;
+    m.row_T = p.row_T;
     if (stage == 1) {
       CUDA_TRY(h, launch_frontend_mfcc_mel(p, ext_max, st));
     } else if (stage == 2) {
@@ -342,6 +350,12 @@ int vp_melspec(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const i
 int vp_mfcc(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep, float* feats,
             float* scratch, void* stream) {
   return run_frontend(h, 1, 1, wave, B, Lpad, keep, feats, scratch, (cudaStream_t)stream);
+}
+
+int vp_features_each(vp_handle* h, const float* wave, int32_t B, int32_t ld, const int32_t* lens, int32_t T, float* feats,
+                     float* scratch, void* stream) {
+  if (!lens) return fail(h, VP_ERR_INVALID, "null argument");
+  return run_frontend(h, -1, -1, wave, B, ld, nullptr, feats, scratch, (cudaStream_t)stream, 0, nullptr, lens, T);
 }
 
 int vp_mfcc_mel(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, float* scratch, float* max_out, void* stream) {

@@ -202,18 +202,26 @@ __global__ void __launch_bounds__(256, 2) frontend_kernel(const __grid_constant_
     cp_async<4>(melidx + 2 * F + i, p.mel_off + i);
   }
   pdl_wait();                 // first access to mutable global memory comes after this
+  // the row's samples and frames: the call's, or in a ragged call the row's own (clamped to the stride and to T)
+  const int L = p.lens ? min(max(p.lens[b], 0), p.L) : p.L;
+  const int T = p.lens ? min(frontend_frames(p.kind, p.frame, WL, N, p.hop, p.kind ? p.pad : 0, L), p.T) : p.T;
+  const int nblk = (T + p.fpb - 1) / p.fpb;
+  if (p.lens) {
+    if (blockIdx.x == 0 && tid == 0) p.row_T[b] = T;
+    if (f0 >= T) { cp_async_wait_all(); return; }   // tiles past the row compute and read nothing
+  }
   // the frame mode maps each staged sample to its source
   const int q0 = f0 * p.hop;
   int i0 = 0;
   if (p.kind == 0 && p.frame != VP_FRAME_KALDI_REFLECT && (reinterpret_cast<size_t>(wv + q0) & 15) == 0) {
-    const int n4 = min(span, p.L - q0) >> 2;        // staged sample i is x[q0 + i]: 16-byte copies while inside the utterance
+    const int n4 = min(span, L - q0) >> 2;        // staged sample i is x[q0 + i]: 16-byte copies while inside the utterance
     for (int i = tid; i < n4; i += 256) cp_async<16>(stage + 4 * i, wv + q0 + 4 * i);
     i0 = n4 * 4;
   }
   for (int i = i0 + tid; i < span; i += 256) {
     int s = q0 + i;
     if (p.kind == 1) {                      // torch.stft of x zero-extended by p.pad at both ends: functional.py:112-134
-      const int Lp = p.L + 2 * p.pad;
+      const int Lp = L + 2 * p.pad;
       if (p.frame != VP_FRAME_STFT_NOCENTER) s -= N / 2;
       if (p.frame == VP_FRAME_DEFAULT) {                  // reflect
         if (s < 0) s = -s;
@@ -228,9 +236,9 @@ __global__ void __launch_bounds__(256, 2) frontend_kernel(const __grid_constant_
     } else if (p.frame == VP_FRAME_KALDI_REFLECT) {       // kaldi._get_strided(snip_edges=False): x[-1-j] / x[2L-1-j]
       s -= p.pad;
       if (s < 0) s = -1 - s;
-      if (s >= p.L) s = 2 * p.L - 1 - s;
+      if (s >= L) s = 2 * L - 1 - s;
     }
-    stage[i] = (s >= 0 && s < p.L) ? __ldg(wv + s) : 0.f;
+    stage[i] = (s >= 0 && s < L) ? __ldg(wv + s) : 0.f;
   }
   cp_async_wait_all();
   __syncthreads();
@@ -244,7 +252,7 @@ __global__ void __launch_bounds__(256, 2) frontend_kernel(const __grid_constant_
   for (int pair = g; pair < npairs; pair += NG) {
     const int fa = f0 + pair * 2;                   // frames packed as real (fa) and imaginary (fa + 1) parts
     const int oa = (fa - f0) * p.hop;
-    const bool va = fa < p.T, vb = fa + 1 < p.T;
+    const bool va = fa < T, vb = fa + 1 < T;
     if (!va) break;                                 // uniform over the group: frames beyond T (last tile of the utterance)
 
     // ---- per-frame mean (kaldi.py:183-186), one warp per frame ----
@@ -453,12 +461,12 @@ __global__ void __launch_bounds__(256, 2) frontend_kernel(const __grid_constant_
 
   const int blk0 = blockIdx.x * p.tpc;              // the CTA's first 16-frame tile
   if (p.cta_max) {
-    // ---- MFCC mel stage: the CTA's maximum, for every tile it owns, for the call-wide top_db clamp
-    // (functional.py:393-399); CMN comes after the DCT
+    // ---- MFCC mel stage: the CTA's maximum, for every tile it owns, for the top_db clamp (functional.py:393-399)
+    // against the call's maximum, or the row's in a ragged call; CMN comes after the DCT
     vmax = warp_max(vmax);
     if ((tid & 31) == 0) red[tid >> 5] = vmax;
     __syncthreads();
-    if (tid < p.tpc && blk0 + tid < p.nblk) {
+    if (tid < p.tpc && blk0 + tid < nblk) {
       float m = red[0];
       for (int i = 1; i < 8; ++i) m = fmaxf(m, red[i]);
       p.cta_max[(size_t)b * p.nblk + blk0 + tid] = m;
@@ -469,17 +477,18 @@ __global__ void __launch_bounds__(256, 2) frontend_kernel(const __grid_constant_
   // features when it fits, else from what this CTA wrote ----
   for (int i = tid; i < p.tpc * F; i += 256) {
     const int ti = i / F, m = i - ti * F;
-    if (blk0 + ti >= p.nblk) break;
+    if (blk0 + ti >= nblk) break;
     const int fb = f0 + ti * p.fpb;
     float s = 0.f;
-    for (int f = fb; f < fb + p.fpb && f < p.T; ++f)
+    for (int f = fb; f < fb + p.fpb && f < T; ++f)
       s += p.cache ? fcache[(size_t)(f - f0) * F + m] : p.feats[((size_t)b * p.T + f) * F + m];
     p.partial[((size_t)b * p.nblk + blk0 + ti) * F + m] = s;
   }
 }
 
 // MFCC tail (torchaudio MFCC.forward): clamp the dB mel values to (max over the WHOLE call) - top_db -- torchaudio folds
-// the batch axis into the clamp's channel axis, so the maximum is shared by every utterance of the call -- then
+// the batch axis into the clamp's channel axis, so the maximum is shared by every utterance of the call; a ragged call
+// (p.row_T) featurizes each row as a call of its own, so a row is clamped against its own tiles' maxima -- then
 // mfcc[t, k] = sum_m mel_db[t, m] * dct[m, k] (create_dct, functional.py:640-667).  One CTA per (frame tile, utterance);
 // also emits the per-CTA column sums that cmn_mask_kernel turns into the CMN mean.
 __global__ void __launch_bounds__(256) mfcc_post_kernel(const __grid_constant__ MfccParams p) {
@@ -493,10 +502,14 @@ __global__ void __launch_bounds__(256) mfcc_post_kernel(const __grid_constant__ 
   const int tid = threadIdx.x;
   const int b = blockIdx.y;
   const int f0 = blockIdx.x * p.fpb;
+  const int T = p.row_T ? p.row_T[b] : p.T;         // frames of the row (its stride stays p.T)
+  if (f0 >= T) return;                              // a tile past a ragged row
   float thr = -INFINITY;
   if (p.top_db >= 0.f) {
+    const float* mx = p.row_T ? p.cta_max + (size_t)b * p.nblk : p.cta_max;
+    const int n_max = p.row_T ? (T + p.fpb - 1) / p.fpb : p.n_max;
     float m = -INFINITY;
-    for (int i = tid; i < p.n_max; i += 256) m = fmaxf(m, __ldg(p.cta_max + i));
+    for (int i = tid; i < n_max; i += 256) m = fmaxf(m, __ldg(mx + i));
     m = warp_max(m);
     if ((tid & 31) == 0) red[tid >> 5] = m;
     __syncthreads();
@@ -508,7 +521,7 @@ __global__ void __launch_bounds__(256) mfcc_post_kernel(const __grid_constant__ 
   for (int i = tid; i < p.fpb * p.M; i += 256) {
     const int fr = i / p.M;
     const int f = f0 + fr;
-    tile[i] = f < p.T ? fmaxf(__ldg(p.mel + ((size_t)b * p.T + f) * p.M + (i - fr * p.M)), thr) : 0.f;
+    tile[i] = f < T ? fmaxf(__ldg(p.mel + ((size_t)b * p.T + f) * p.M + (i - fr * p.M)), thr) : 0.f;
   }
   __syncthreads();
   for (int i = tid; i < p.fpb * p.K; i += 256) {
@@ -518,28 +531,32 @@ __global__ void __launch_bounds__(256) mfcc_post_kernel(const __grid_constant__ 
     float s = 0.f;
     for (int m = 0; m < p.M; ++m) s = fmaf(row[m], dct[m * p.K + k], s);
     outt[i] = s;
-    if (f0 + fr < p.T) p.feats[((size_t)b * p.T + f0 + fr) * p.K + k] = s;
+    if (f0 + fr < T) p.feats[((size_t)b * p.T + f0 + fr) * p.K + k] = s;
   }
   __syncthreads();
   for (int k = tid; k < p.K; k += 256) {
     float s = 0.f;
-    for (int fr = 0; fr < p.fpb && f0 + fr < p.T; ++fr) s += outt[fr * p.K + k];
+    for (int fr = 0; fr < p.fpb && f0 + fr < T; ++fr) s += outt[fr * p.K + k];
     p.partial[((size_t)b * p.nblk + blockIdx.x) * p.K + k] = s;
   }
 }
 
 // feats[b, t, :] -= mean_t(feats[b]) over ALL T frames, then frames t >= keep[b] are zeroed (featurizer.py:79-90).
+// Ragged call (row_T non-null): row b's mean is over its own row_T[b] frames (the first row_T[b] / fpb tiles' partial
+// sums) and frames t >= row_T[b] are zeroed -- collate_fn's zero padding of a singly featurized utterance.
 __global__ void __launch_bounds__(128) cmn_mask_kernel(float* feats, const float* partial, const int* keep, int T, int F,
-                                                       int nblk, int rows_per_cta) {
+                                                       int nblk, int rows_per_cta, const int* row_T, int fpb) {
   pdl_launch_dependents();
   pdl_wait();                 // first access to mutable global memory comes after this
   const int b = blockIdx.y;
-  const int kp = keep ? keep[b] : T;
+  const int Tb = row_T ? row_T[b] : T;
+  const int nb = row_T ? (Tb + fpb - 1) / fpb : nblk;
+  const int kp = keep ? keep[b] : Tb;
   const int t0 = blockIdx.x * rows_per_cta;
   for (int m = threadIdx.x; m < F; m += blockDim.x) {        // F > 128 only for Spectrogram (n_fft/2 + 1 bins)
     float s = 0.f;
-    for (int i = 0; i < nblk; ++i) s += partial[((size_t)b * nblk + i) * F + m];
-    const float mean = s / (float)T;
+    for (int i = 0; i < nb; ++i) s += partial[((size_t)b * nblk + i) * F + m];
+    const float mean = s / (float)Tb;
     const int t1 = min(t0 + rows_per_cta, T);
     for (int tb = t0; tb < t1; tb += 16) {                   // 16 rows in flight: all their loads, then their stores
       float v[16];
@@ -681,7 +698,7 @@ cudaError_t launch_frontend_mfcc_finish(const FrontendParams& p, const MfccParam
   if (e != cudaSuccess) return e;
   const int rows = 64;
   dim3 g2((p.T + rows - 1) / rows, p.B);
-  launch_pdl(cmn_mask_kernel, g2, 128, 0, stream, m.feats, m.partial, keep, p.T, m.K, p.nblk, rows);
+  launch_pdl(cmn_mask_kernel, g2, 128, 0, stream, m.feats, m.partial, keep, p.T, m.K, p.nblk, rows, m.row_T, p.fpb);
   return cudaGetLastError();
 }
 
@@ -698,7 +715,7 @@ cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream
   if (e != cudaSuccess) return e;
   const int rows = 64;
   dim3 g2((p.T + rows - 1) / rows, p.B);
-  launch_pdl(cmn_mask_kernel, g2, 128, 0, stream, p.feats, p.partial, keep, p.T, p.F, p.nblk, rows);
+  launch_pdl(cmn_mask_kernel, g2, 128, 0, stream, p.feats, p.partial, keep, p.T, p.F, p.nblk, rows, p.row_T, p.fpb);
   return cudaGetLastError();
 }
 

@@ -17,7 +17,21 @@ struct FrontendParams {
   float* cta_max;      // non-null: MFCC mel stage (per-CTA maxima instead of CMN partial sums)
   int n_pass, radix[12], G;   // FFT pass plan + threads per FFT group (frontend_plan)
   int tpc, cache;             // fpb-frame tiles per CTA; 1: the CTA keeps its features in shared memory for the sums
+  // Ragged call (vp_features_each): non-null lens[b] = samples of row b (L is then only the row stride); every row is
+  // framed as a call of its own and its frame count T_b (frontend_frames, at most T) goes to row_T[b].
+  const int* lens; int* row_T;
 };
+// Frames of an n-sample signal (vp_num_frames): kind 0 snip_edges / half-sample reflection, kind 1 torch.stft of the
+// signal zero-extended by stft_pad at both ends, centred or not.
+__host__ __device__ inline int frontend_frames(int kind, int frame, int win, int n_fft, int hop, int stft_pad, int64_t n) {
+  if (kind == 0) {
+    if (frame == VP_FRAME_KALDI_REFLECT) return (int)((n + hop / 2) / hop);
+    return n < win ? 0 : (int)(1 + (n - win) / hop);
+  }
+  const int64_t Lp = n + 2 * (int64_t)stft_pad;
+  if (frame == VP_FRAME_STFT_NOCENTER) return Lp < n_fft ? 0 : (int)(1 + (Lp - n_fft) / hop);
+  return (int)(1 + Lp / hop);
+}
 // fills the line above from the shape fields (no pointer is read); mfcc_mel: the MFCC mel stage (maxima, no CMN sums)
 void frontend_plan(FrontendParams& p, bool mfcc_mel);
 void frontend_twiddle_table(int N, const double2* tw, double2* out);
@@ -36,6 +50,7 @@ struct MfccParams {
   const float* mel; const float* cta_max; const float* dct; float* feats; float* partial;
   int B, T, M, K, fpb, nblk, n_max;
   float top_db;        // < 0: no clamp
+  const int* row_T;    // non-null: ragged call, row b has row_T[b] frames and is clamped against its own maximum
 };
 
 struct StatsParams {
@@ -106,6 +121,7 @@ cudaError_t launch_flac_decode(const uint8_t* data, int64_t nbytes, const int64_
 cudaError_t launch_pcm_decode(const uint8_t* data, int64_t nbytes, const vp_pcm_info* info, int B, float* out,
                               int64_t ld, int32_t* status, cudaStream_t stream);
 
+// keep: frames kept per row (the rest zeroed), or null; a ragged call (p.lens) keeps each row's own T_b instead
 cudaError_t launch_frontend(const FrontendParams& p, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc(const FrontendParams& p, const MfccParams& m, const int* keep, cudaStream_t stream);
 cudaError_t launch_frontend_mfcc_mel(const FrontendParams& p, float* max_out, cudaStream_t stream);

@@ -101,6 +101,7 @@ def lib():
         'vp_fbank': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
         'vp_melspec': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
         'vp_mfcc': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
+        'vp_features_each': (C.c_int, [vp, f32p, i32, i32, i32p, i32, f32p, f32p, vp]),
         'vp_mfcc_mel': (C.c_int, [vp, f32p, i32, i32, f32p, f32p, vp]),
         'vp_mfcc_finish': (C.c_int, [vp, i32, i32, i32p, f32p, f32p, f32p, vp]),
         'vp_frontend_plan_info': (C.c_int, [vp, i32, i32, i32, i32p]),
@@ -162,7 +163,7 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_feature_dim',
            'vp_weights_load', 'vp_program_create', 'vp_program_destroy', 'vp_embed', 'vp_embed_wave',
            'vp_program_launches', 'vp_program_peek', 'vp_embed_profiled', 'vp_program_op_info', 'vp_host_gather_pad',
-           'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_frontend_plan_info', 'vp_cosine_scores', 'vp_device_zero',
+           'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_features_each', 'vp_frontend_plan_info', 'vp_cosine_scores', 'vp_device_zero',
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
            'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics',
            'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize', 'vp_frame_energy', 'vp_gather_windows',

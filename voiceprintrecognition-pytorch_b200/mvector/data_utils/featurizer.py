@@ -488,6 +488,40 @@ class AudioFeaturizer:
                                        self._engine.stream_ptr()))
         return feats
 
+    def forward_each(self, w, lens):
+        """Every row of a ragged batch featurized as if it were the whole call (vp_features_each): the reference's
+        eval / feature-extraction mode, where each file is featurized alone (reader.py:82-107) and the features are then
+        zero-padded to the longest (collate_fn.py:5-24).  ``w`` CUDA float32 [B, ld] contiguous, row b holding ``lens[b]``
+        samples (host ints).  -> (feats CUDA [B, T, F], T the longest row's frames, row b +0.0 past its own frames;
+        T_b numpy int32 [B]).  A row the one-row call would refuse raises that call's error: forward_keep's
+        AssertionError for a Kaldi row shorter than the window, the library's length error for an STFT row."""
+        self._ensure()
+        B, ld = w.shape
+        lens = np.asarray(lens, dtype=np.int64).reshape(-1)
+        assert lens.size == B and (lens >= 0).all() and (lens <= ld).all(), 'one length in [0, ld] per row'
+        lib = L.lib()
+        h = self._engine.handle
+        # Every length rule of the library (window, padding, at least one frame) holds for all lengths from some minimum
+        # up, so the shortest row is the one to check: the library's host-only plan query refuses it exactly when a
+        # one-row call would, and that one-row call then raises its own error before any launch.
+        short = int(np.argmin(lens))
+        info = (C.c_int32 * 8)()
+        if lib.vp_frontend_plan_info(h, 1, int(lens[short]), self.feat_fun.desc.post, info) != L.VP_OK:
+            self.forward_keep(w[short:short + 1, :int(lens[short])].contiguous())
+            raise RuntimeError(f'row {short} of {int(lens[short])} samples is refused by the front-end')
+        tb = np.array([self.num_frames(n) for n in lens.tolist()], dtype=np.int32)
+        T = int(tb.max())
+        dev = self._engine.device
+        feats = torch.empty(B, T, self.feature_dim, dtype=torch.float32, device=dev)
+        # the call's own scratch: sized by the longest row, not by the stride
+        scratch = torch.empty(max(int(lib.vp_frontend_scratch_floats(h, B, int(lens.max()))), 1), dtype=torch.float32,
+                              device=dev)
+        lens_dev = torch.from_numpy(lens.astype(np.int32)).to(dev, non_blocking=True)
+        _check(h, lib.vp_features_each(h, C.c_void_p(w.data_ptr()), B, ld, C.c_void_p(lens_dev.data_ptr()), T,
+                                       C.c_void_p(feats.data_ptr()), C.c_void_p(scratch.data_ptr()),
+                                       self._engine.stream_ptr()))
+        return feats, tb
+
     def mfcc_sharded(self, w, B, Lp, kp, feats, scratch, stream, group):
         """MFCC of this rank's shard of ONE sharded call: vp_mfcc_mel -> all-reduce(MAX) of the clamp maximum over
         ``group`` -> vp_mfcc_finish, all enqueued on ``stream``.  Bit-identical to the single-process vp_mfcc of the whole
