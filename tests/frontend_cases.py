@@ -138,8 +138,29 @@ def _log(d, s):
     return s
 
 
-def exact_features(method, args, x, keep=None):
+def warp_frame_mean(frames):
+    """The kernel's per-frame mean (frontend.cu, remove_dc): fp32 partial sums of the samples j = lane, lane + 32, ...
+    in order, the 32 partials reduced by warp_sum's xor butterfly (common.cuh), divided by the frame length in fp32.
+    After DC removal the weak low bins see little but the mean's own rounding: on tests/frontend_each_cases.py's rows,
+    another rounding of the mean alone moves the reference by up to 1.3e-4 log units there.
+    frames [m, size] float32 tensor -> [m, 1]."""
+    f = frames.numpy()
+    m, size = f.shape
+    f = np.pad(f, ((0, 0), (0, -size % 32))).reshape(m, -1, 32)
+    p = np.zeros((m, 32), np.float32)
+    for k in range(f.shape[1]):
+        p = p + f[:, k]
+    lanes = np.arange(32)
+    for o in (16, 8, 4, 2, 1):
+        p = p + p[:, lanes ^ o]
+    return torch.from_numpy(p[:, :1] / np.float32(size))
+
+
+def exact_features(method, args, x, keep=None, frame_mean=None):
     """One AudioFeaturizer call on x [B, Lpad] float32 -> (features [B, T, F] float64, scale [B, T]).
+
+    ``frame_mean``: the Kaldi kind's per-frame DC offset in fp32 (None: torch's mean; warp_frame_mean: the kernel's
+    summation order, which the weak low bins after DC removal are sensitive to).
 
     ``scale`` is what the fp32 roundings of a frame's row are proportional to: the largest magnitude before CMN in that
     frame or in the CMN means it is shifted by (for Mel / Spectrogram: the frame maximum).  ``keep`` [B] frames kept
@@ -149,8 +170,8 @@ def exact_features(method, args, x, keep=None):
     d = f.desc
     if d.kind == 0:
         # kaldi.fbank: fp32 framing / DC / pre-emphasis / window, fp64 FFT, power and projection rounded to fp32 once
-        mel = np.stack([ofo.kaldi_fbank(torch.from_numpy(r), exact_spectrum=True, **dict(args, use_log_fbank=False))
-                        .numpy() for r in x])
+        mel = np.stack([ofo.kaldi_fbank(torch.from_numpy(r), exact_spectrum=True, frame_mean=frame_mean,
+                                        **dict(args, use_log_fbank=False)).numpy() for r in x])
     else:
         mel = stft_mel(f, x)
     pre = _log(d, mel)

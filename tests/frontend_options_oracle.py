@@ -25,9 +25,10 @@ def kaldi_frames(w, size, shift, snip_edges):
     return ext.as_strided((m, size), (shift, 1))
 
 
-def kaldi_fbank(waveform, exact_spectrum=False, **kwargs):
+def kaldi_fbank(waveform, exact_spectrum=False, frame_mean=None, **kwargs):
     """One utterance -> [m, num_mel_bins]; ``exact_spectrum`` as in oracle.frontend.kaldi_fbank (fp64 FFT, power and
-    projection on the same fp32 frames)."""
+    projection on the same fp32 frames).  ``frame_mean``: frames [m, size] float32 -> their DC offsets [m, 1] float32
+    (default torch's mean)."""
     from mvector.data_utils.featurizer import kaldi_mel_banks
     a = ofe.fbank_args(**kwargs)
     if a['dither'] != 0.0 or a['use_energy'] or a['min_duration'] != 0.0:
@@ -38,7 +39,7 @@ def kaldi_fbank(waveform, exact_spectrum=False, **kwargs):
     assert 2 <= size <= w.numel()
     frames = kaldi_frames(w, size, shift, a['snip_edges'])
     if a['remove_dc_offset']:
-        frames = frames - frames.mean(dim=1, keepdim=True)
+        frames = frames - (frames.mean(dim=1, keepdim=True) if frame_mean is None else frame_mean(frames))
     c = a['preemphasis_coefficient']
     if c != 0.0:
         frames = frames - c * torch.cat([frames[:, :1], frames[:, :-1]], dim=1)
