@@ -24,7 +24,8 @@ The arithmetic model (u = 2^-24, one fp32 round-to-nearest operation):
     bound stays a bound), activations add their Lipschitz constant times the incoming bound plus the CUDA Math API ulp
     bound of expf / tanhf (2 ulp each; the build has no fast-math flags); input error propagates as |W| beta_in;
   * copies, padding and max pooling are exact.
-Every buffer the interpreter stores is rounded to fp32 as the GPU's is, which adds u |v| to the stored bound."""
+Every buffer the interpreter stores is rounded to fp32 as the GPU's is, which adds max(u |v|, 2^-150) to the stored
+bound (``stored``: u |v| for normal values, half an ulp of the subnormals below them)."""
 import numpy as np
 
 import op_cases as oc
@@ -32,10 +33,16 @@ from mvector import _lib as L
 from plan_sim import Sim, _act
 
 U = 2.0 ** -24
+SUB = 2.0 ** -150                    # half the spacing of fp32 subnormals: the rounding error of a store below 2^-126
 TRUNC = 2.0 ** -23
 TF32_RHO, TF32_LAM, TF32_FLUSH = 2.0 ** -21, 2.0 ** -11, 2.0 ** -126
 F16_RHO, F16_LAM, F16_FLOOR = 2.0 ** -22, 2.0 ** -11, 2.0 ** -25
 ELEMS = 1 << 22                      # working-set target (fp64 elements) of one row block
+
+
+def stored(v):
+    """The rounding error bound of storing the fp64 value v as fp32."""
+    return np.maximum(U * np.abs(v), SUB)
 
 
 def kernel_scale_exp(amax, lo=-114, hi=126):
@@ -84,11 +91,13 @@ def act_bound(v, b, act):
     raise ValueError(act)
 
 
-def chain_abs(A, W, step, group=1):
+def chain_abs(A, W, step, group=1, r_full=None):
     """Sequential accumulation of sum_k A[:, k] W[:, k], one partial sum per ``step`` columns: -> (an upper bound on the
     sum over all partials of |partial| [r, N], the final sum [r, N]).  The partials are computed (in fp32: this is a
     bound, and fp32's error is far below the 2^-10 margin applied) at the end of every ``group`` steps; a partial inside
-    a group is within the group's |products| of both ends, so |P_j| <= (|P_start| + |P_end| + sum_group |p|) / 2."""
+    a group is within the group's |products| of both ends, so |P_j| <= (|P_start| + |P_end| + sum_group |p|) / 2.
+    ``r_full``: the row count that sets how many K blocks are summed per batch (default r): a subset of a row block
+    passes the block's own count, so that its K blocks are grouped as the whole block's are."""
     r, K = A.shape
     N = W.shape[0]
     blk = step * group
@@ -101,7 +110,7 @@ def chain_abs(A, W, step, group=1):
     ends = np.zeros((r, N), dtype=np.float32)                 # sum over blocks of |P_end|
     starts = np.zeros((r, N), dtype=np.float32)               # sum over blocks of |P_start|
     P = np.zeros((r, N), dtype=np.float32)
-    per = max(1, ELEMS // (r * N))
+    per = max(1, ELEMS // ((r if r_full is None else r_full) * N))
     for j0 in range(0, nb, per):
         T = np.matmul(Ar[j0:j0 + per], Wr[j0:j0 + per])
         T[0] += P
@@ -116,7 +125,7 @@ def chain_abs(A, W, step, group=1):
     return S * (1 + 2.0 ** -10), P.astype(np.float64)
 
 
-def ffma_chain_bound(A, W, o):
+def ffma_chain_bound(A, W, o, r_full=None):
     """u x sum |partial| of the FFMA kernels' accumulation order (conv_ffma.cu): linear_small_m's 32 lane chains (lane l
     takes k = 128 j + 4 l .. + 3) and its xor butterfly; every other FFMA kernel runs k in order."""
     if oc.kernel_of(o, L.ENGINE_FFMA) == 'linear_small_m':
@@ -128,7 +137,7 @@ def ffma_chain_bound(A, W, o):
         lane_sums = []
         for ln in range(32):
             a, w = Ap[:, :, ln].reshape(r, -1), Wp[:, :, ln].reshape(W.shape[0], -1)
-            S, _ = chain_abs(a, w, 1, 4)
+            S, _ = chain_abs(a, w, 1, 4, r_full)
             tot = tot + S
             lane_sums.append(a @ w.T)
         g = np.stack(lane_sums)                                   # [32, r, N]
@@ -136,11 +145,11 @@ def ffma_chain_bound(A, W, o):
             g = g[0::2] + g[1::2]
             tot = tot + np.abs(g).sum(0)
         return U * tot
-    S, _ = chain_abs(A, W, 1, 16)
+    S, _ = chain_abs(A, W, 1, 16, r_full)
     return U * S
 
 
-def tc_acc_bound(A, W, o, engine):
+def tc_acc_bound(A, W, o, engine, r_full=None):
     """Truncating accumulation of a tensor-core conv: 2^-23 (sum over updates of |acc in| + |acc out|) in the kernel's K
     order (K step 8 / 16, three updates per step, accumulation chunks of tc_schedule's kc K blocks restarting from zero),
     2^-23 x 4 sum |a||w| for the updates' products, and u |running sum| for every chunk fold."""
@@ -152,7 +161,7 @@ def tc_acc_bound(A, W, o, engine):
     run = 0.0
     fold = 0.0
     for c, k0 in enumerate(range(0, K, chunk)):
-        S, Pn = chain_abs(A[:, k0:k0 + chunk], W[:, k0:k0 + chunk], step, 4)
+        S, Pn = chain_abs(A[:, k0:k0 + chunk], W[:, k0:k0 + chunk], step, 4, r_full)
         Pn = np.abs(Pn)
         # per step j: updates (P_{j-1} + ..), (.. + ..), -> P_j; |in| + |out| <= 5 |P_{j-1}| + |P_j| (the lo terms'
         # contributions inside a step are in the 4 sum |a||w| above); P_0 = 0
@@ -177,9 +186,127 @@ def split_bound(A, W, o, engine, s):
     return lA @ lW.T + c * (rA @ aW.T + aA @ rW.T)
 
 
+def views(o):
+    """The views a lowered op reads and writes: name -> (off, ld, coff, C, rows).  Operands: 'src', 'src2', 'res',
+    'gate', 'ubias' and 'sum' (the accumulate-into view's prior); outputs: 'dst' and 'sum'.  Only the views the op uses
+    are listed."""
+    v = {}
+    rows_in = o.B * o.Tin * o.Fin
+    if o.kind in (L.OP_CONV, L.OP_CONV_C1):
+        M = o.B * o.Tout * o.Fout
+        v['src'] = (o.src, o.in_ld, o.in_coff, o.Cin, rows_in)
+        if o.src2_mode != L.SRC2_NONE:
+            v['src2'] = (o.src2, o.src2_ld, o.src2_coff, o.Cin2 if o.src2_mode == L.SRC2_CONCAT else o.Cin, rows_in)
+        if o.res != L.BUF_NONE:
+            v['res'] = (o.res, o.res_ld, o.res_coff, o.Cout, M)
+        for f in ('gate', 'ubias'):
+            if getattr(o, f) != L.BUF_NONE:
+                v[f] = (getattr(o, f), o.Cout, 0, o.Cout, o.B * o.n_seg)
+        if o.sum != L.BUF_NONE:
+            v['sum'] = (o.sum, o.sum_ld, o.sum_coff, o.Cout, M)
+        v['dst'] = (o.dst, o.out_ld, o.out_coff, o.Cout, M)
+    elif o.kind == L.OP_EW:
+        v['src'] = (o.src, o.in_ld, o.in_coff, o.Cin, rows_in)
+        if o.mode == L.EW_GATE_RES and o.gate != L.BUF_NONE:
+            v['gate'] = (o.gate, o.Cin, 0, o.Cin, o.B)
+        if o.mode in (L.EW_GATE_RES, L.EW_AFF) and o.res != L.BUF_NONE:
+            v['res'] = (o.res, o.res_ld, o.res_coff, o.Cin, rows_in)
+        if o.mode == L.EW_AFF:
+            v['src2'] = (o.src2, o.src2_ld, o.src2_coff, o.Cin, rows_in)
+        v['dst'] = (o.dst, o.out_ld, o.out_coff, o.Cout if o.mode == L.EW_PAD_COPY else o.Cin, rows_in)
+    elif o.kind == L.OP_POOL2D:
+        v['src'] = (o.src, o.in_ld, o.in_coff, o.Cin, rows_in)
+        v['dst'] = (o.dst, o.out_ld, o.out_coff, o.Cin, o.B * o.Tout * o.Fout)
+    elif o.kind == L.OP_COLSTATS:
+        v['src'] = (o.src, o.in_ld, o.in_coff, o.Cin, rows_in)
+        seg = o.mode == L.STATS_SEG_CONTEXT
+        v['dst'] = (o.dst, o.out_ld, o.out_coff, o.Cin if seg or o.mode == L.STATS_MEAN else 2 * o.Cin,
+                    o.B * (o.n_seg if seg else 1))
+    elif o.kind == L.OP_ASP_POOL:
+        v['src'] = (o.src, o.in_ld, o.in_coff, o.Cin, o.B * o.Tin)
+        v['src2'] = (o.src2, o.src2_ld, o.src2_coff, o.Cin, o.B * o.Tin)
+        v['dst'] = (o.dst, o.out_ld, o.out_coff, o.Cin if o.mode == 1 else 2 * o.Cin, o.B)
+    else:
+        raise ValueError(o.kind)
+    return v
+
+
+def conv_taps(o, m):
+    """Input rows of every tap of a conv's output rows m: [(tap, row, ok)] in (kt, kf) order, rows clipped into the
+    map and ok False where the tap falls in zero padding (the row is then read and multiplied by 0)."""
+    b = m // (o.Tout * o.Fout)
+    to = (m // o.Fout) % o.Tout
+    fo = m % o.Fout
+    out = []
+    for kt in range(o.KT):
+        for kf in range(o.KF):
+            ti = to * o.sT - o.padT + kt * o.dT
+            fi = fo * o.sF - o.padF + kf * o.dF
+            if o.pad_mode == L.PAD_REFLECT:
+                ti = np.where(ti < 0, -ti, ti)
+                ti = np.where(ti >= o.Tin, 2 * (o.Tin - 1) - ti, ti)
+            ok = (ti >= 0) & (ti < o.Tin) & (fi >= 0) & (fi < o.Fin)
+            row = (b * o.Tin + np.clip(ti, 0, o.Tin - 1)) * o.Fin + np.clip(fi, 0, o.Fin - 1)
+            out.append((kt * o.KF + kf, row, ok))
+    return out
+
+
+def pool_windows(o, m):
+    """Windows of pool2d output rows m, grouped by output position: [(rows of m at (to, fo), input rows [n, window])]
+    with the window in (kt, kf) order, clipped to the map (count_include_pad: the divisor stays KT KF)."""
+    b = m // (o.Tout * o.Fout)
+    pos = m % (o.Tout * o.Fout)
+    out = []
+    for p in np.unique(pos):
+        to, fo = divmod(int(p), o.Fout)
+        t0, f0 = to * o.sT - o.padT, fo * o.sF - o.padF
+        ts = np.arange(max(t0, 0), min(t0 + o.KT, o.Tin))
+        fs = np.arange(max(f0, 0), min(f0 + o.KF, o.Fin))
+        sel = pos == p
+        win = ((b[sel, None, None] * o.Tin + ts[None, :, None]) * o.Fin + fs[None, None, :]).reshape(int(sel.sum()), -1)
+        out.append((sel, win))
+    return out
+
+
+def operand_rows(o, m):
+    """Rows of each operand view that the outputs rows m of op o depend on: name -> sorted row indices."""
+    v = views(o)
+    need = {}
+    if o.kind in (L.OP_CONV, L.OP_CONV_C1):
+        rows = np.unique(np.concatenate([r for _, r, _ in conv_taps(o, m)]))
+        need['src'] = rows
+        if 'src2' in v:
+            need['src2'] = rows
+        for f in ('gate', 'ubias'):
+            if f in v:
+                need[f] = np.arange(v[f][4])
+        for f in ('res', 'sum'):
+            if f in v:
+                need[f] = m
+    elif o.kind == L.OP_EW:
+        for f in ('src', 'src2', 'res'):
+            if f in v:
+                need[f] = m
+        if 'gate' in v:
+            need['gate'] = np.arange(o.B)
+    elif o.kind == L.OP_POOL2D:
+        need['src'] = np.unique(np.concatenate([w.reshape(-1) for _, w in pool_windows(o, m)]))
+    else:                                                          # colstats / asp: every row
+        for f in ('src', 'src2'):
+            if f in v:
+                need[f] = np.arange(v[f][4])
+    return need
+
+
 class BoundSim(Sim):
     """plan_sim.Sim carrying a per-element bound on |GPU - fp64| next to every value.  ``engines``: the resolved engine of
-    every op (op_cases.engine_of / program_engines); ``mutate``: see test_error_bound_cpu.py (None here)."""
+    every op (op_cases.engine_of / program_engines).
+
+    Each op method takes the op and, optionally, ``rows`` (the output rows to compute, default all), ``read`` (a
+    function (name, rows) -> (values, bounds) [len(rows), C] of the operand view ``name`` of ``views``, default the
+    interpreter's own workspace) and ``s`` (the fp16 split's scale exponent, default the design exponent of the source
+    the interpreter holds).  It returns {'dst': (values, bounds)} and, for an accumulate-into conv, 'sum'; with
+    ``rows`` None it also stores them, as run() does."""
 
     def __init__(self, pb, blob, feats, engines=None):
         super().__init__(pb, blob, feats)
@@ -188,6 +315,14 @@ class BoundSim(Sim):
         self.binp = np.zeros(self.inp.size)
         ops = pb.finalize().ops if engines is None else None
         self.engines = engines if engines is not None else [oc.engine_of(op) for op in ops]
+
+    @classmethod
+    def for_ops(cls, pb, blob, engines):
+        """An instance without memory of its own, for ``op`` on operands from an explicit reader (a program's
+        workspace can be far larger than the rows one op's reference needs)."""
+        self = cls.__new__(cls)
+        self.pb, self.blob, self.engines = pb, np.asarray(blob, dtype=np.float32), engines
+        return self
 
     def _bmem(self, off):
         if off == L.BUF_INPUT:
@@ -204,7 +339,19 @@ class BoundSim(Sim):
         super().wr(off, rows, ld, coff, C, val)
         mem, base = self._bmem(off)
         b = np.zeros(val.shape) if beta is None else beta
-        mem[base + (np.arange(rows)[:, None] * ld + coff + np.arange(C)[None, :])] = b if exact else b + U * np.abs(val)
+        mem[base + (np.arange(rows)[:, None] * ld + coff + np.arange(C)[None, :])] = b if exact else b + stored(val)
+
+    def reader(self, o):
+        """The workspace reader of op o: (name, rows) -> the values and bounds the interpreter holds."""
+        v = views(o)
+
+        def read(name, rows):
+            off, ld, coff, C, _ = v[name]
+            mem, base = self._mem(off)
+            bmem, bbase = self._bmem(off)
+            idx = rows[:, None] * ld + coff + np.arange(C)[None, :]
+            return mem[base + idx].astype(np.float64), bmem[bbase + idx]
+        return read
 
     def run(self):
         for self.i, o in enumerate(self.pb.ops):
@@ -213,18 +360,26 @@ class BoundSim(Sim):
         assert not np.isnan(self.out).any(), 'program output not fully written'
         return self.out.copy(), self.bout.copy()
 
+    def _store(self, o, out):
+        """Write an op's outputs (bounds with their store rounding) into the interpreter's memory."""
+        v = views(o)
+        for name, (val, b) in out.items():
+            off, ld, coff, C, rows = v[name]
+            self.wr(off, rows, ld, coff, C, val, b, exact=True)
+        return out
+
     # ------------------------------------------------------------------
-    def _operand(self, o):
-        """The conv's gathered source map [rows_in, cin_tot] and its bound (the add / prologue rounded once)."""
-        X = self.rd(o.src, o.B * o.Tin * o.Fin, o.in_ld, o.in_coff, o.Cin)
-        bX = self.rdb(o.src, o.B * o.Tin * o.Fin, o.in_ld, o.in_coff, o.Cin)
-        rows_in = o.B * o.Tin * o.Fin
+    def _operand(self, o, read, rows):
+        """The conv's gathered source rows [len(rows), cin_tot] and their bound (the add / prologue rounded once)."""
+        X, bX = read('src', rows)
         if o.src2_mode == L.SRC2_ADD:
-            X = X + self.rd(o.src2, rows_in, o.src2_ld, o.src2_coff, o.Cin)
-            bX = bX + self.rdb(o.src2, rows_in, o.src2_ld, o.src2_coff, o.Cin) + U * np.abs(X)
+            Y, bY = read('src2', rows)
+            X = X + Y
+            bX = bX + bY + U * np.abs(X)
         elif o.src2_mode == L.SRC2_CONCAT:
-            X = np.concatenate([X, self.rd(o.src2, rows_in, o.src2_ld, o.src2_coff, o.Cin2)], axis=1)
-            bX = np.concatenate([bX, self.rdb(o.src2, rows_in, o.src2_ld, o.src2_coff, o.Cin2)], axis=1)
+            Y, bY = read('src2', rows)
+            X = np.concatenate([X, Y], axis=1)
+            bX = np.concatenate([bX, bY], axis=1)
         if o.pre_s >= 0:
             cin_tot = X.shape[1]
             s = self.w(o.pre_s, cin_tot)[None]
@@ -234,55 +389,54 @@ class BoundSim(Sim):
                 X = np.maximum(X, 0)
         return X, bX
 
-    def _im2col(self, X, bX, o, m, taps=None):
-        """Rows m of the implicit-GEMM operand [len(m), K] (K ordered (tap, ci)) and its bound; padding is exact 0."""
-        b = m // (o.Tout * o.Fout)
-        to = (m // o.Fout) % o.Tout
-        fo = m % o.Fout
+    @staticmethod
+    def _im2col(X, bX, o, m, taps=None, in_rows=None):
+        """Rows m of the implicit-GEMM operand [len(m), K] (K ordered (tap, ci)) and its bound; padding is exact 0.
+        ``in_rows``: the input rows X holds (default all, in order)."""
         A, bA = [], []
-        for kt in range(o.KT):
-            for kf in range(o.KF):
-                if taps is not None and kt * o.KF + kf not in taps:
-                    continue
-                ti = to * o.sT - o.padT + kt * o.dT
-                fi = fo * o.sF - o.padF + kf * o.dF
-                if o.pad_mode == L.PAD_REFLECT:
-                    ti = np.where(ti < 0, -ti, ti)
-                    ti = np.where(ti >= o.Tin, 2 * (o.Tin - 1) - ti, ti)
-                ok = ((ti >= 0) & (ti < o.Tin) & (fi >= 0) & (fi < o.Fin))[:, None]
-                row = (b * o.Tin + np.clip(ti, 0, o.Tin - 1)) * o.Fin + np.clip(fi, 0, o.Fin - 1)
-                A.append(X[row] * ok)
-                bA.append(bX[row] * ok)
+        for t, row, ok in conv_taps(o, m):
+            if taps is not None and t not in taps:
+                continue
+            if in_rows is not None:
+                row = np.searchsorted(in_rows, row)
+            A.append(X[row] * ok[:, None])
+            bA.append(bX[row] * ok[:, None])
         return np.concatenate(A, 1), np.concatenate(bA, 1)
 
-    def conv(self, o):
+    def conv(self, o, rows=None, read=None, s=None):
         eng = self.engines[self.i] if o.kind == L.OP_CONV else L.ENGINE_FFMA
         M = o.B * o.Tout * o.Fout
-        X, bX = self._operand(o)
+        keep_ws = read is None
+        read = read or self.reader(o)
+        m = np.arange(M) if rows is None else np.asarray(rows)
+        in_rows = None if rows is None else operand_rows(o, m)['src']
+        X, bX = self._operand(o, read, np.arange(o.B * o.Tin * o.Fin) if in_rows is None else in_rows)
         K = o.KT * o.KF * X.shape[1]
         W = self.wmat(o.w, o.Cout, o.w_ld, K)
-        s = design_scale_exp(np.abs(X).max()) if eng == L.ENGINE_TC16 else 0
-        acc = np.zeros((M, o.Cout))
+        if s is None:
+            s = design_scale_exp(np.abs(X).max()) if eng == L.ENGINE_TC16 else 0
+        acc = np.zeros((len(m), o.Cout))
         for t in range(o.KT * o.KF):                               # the value exactly as Sim.conv sums it: tap by tap
-            A, _ = self._im2col(X, bX, o, np.arange(M), taps=[t])
+            A, _ = self._im2col(X, bX, o, m, taps=[t], in_rows=in_rows)
             acc += A @ W[:, t * X.shape[1]:(t + 1) * X.shape[1]].T
-        bacc = np.zeros((M, o.Cout))
+        bacc = np.zeros((len(m), o.Cout))
         rb = max(1, min(M, ELEMS // max(K, o.Cout * 8)))
         aW = np.abs(W)
-        for r0 in range(0, M, rb):
-            m = np.arange(r0, min(M, r0 + rb))
-            A, bA = self._im2col(X, bX, o, m)
+        blk = m // rb                                              # the row block of the full op each row falls in
+        for j in np.unique(blk):
+            sel = np.flatnonzero(blk == j)
+            r_full = min(M, (j + 1) * rb) - j * rb
+            A, bA = self._im2col(X, bX, o, m[sel], in_rows=in_rows)
             b = bA @ aW.T
             if eng in (L.ENGINE_TC, L.ENGINE_TC16):
-                b += split_bound(A, W, o, eng, s) + tc_acc_bound(A, W, o, eng)
+                b += split_bound(A, W, o, eng, s) + tc_acc_bound(A, W, o, eng, r_full)
             else:
-                b += ffma_chain_bound(A, W, o)
-            bacc[m] = b
-        self._epilogue(o, eng, acc, bacc)
+                b += ffma_chain_bound(A, W, o, r_full)
+            bacc[sel] = b
+        out = self._epilogue(o, eng, acc, bacc, m, read)
+        return self._store(o, out) if rows is None and keep_ws else out
 
-    def _epilogue(self, o, eng, v, b):
-        M = o.B * o.Tout * o.Fout
-        m = np.arange(M)
+    def _epilogue(self, o, eng, v, b, m, read):
         seg = np.minimum(((m // o.Fout) % o.Tout) // o.seg_len, o.n_seg - 1)
         urow = m // (o.Tout * o.Fout) * o.n_seg + seg
         if o.bias >= 0:
@@ -290,28 +444,31 @@ class BoundSim(Sim):
         if o.bias >= 0 or eng == L.ENGINE_TC16:          # acc + bias (tensor cores: fmaf(acc, descale, bias))
             b = b + U * np.abs(v)
         if o.ubias != L.BUF_NONE:
-            v = v + self.rd(o.ubias, o.B * o.n_seg, o.Cout, 0, o.Cout)[urow]
-            b = b + self.rdb(o.ubias, o.B * o.n_seg, o.Cout, 0, o.Cout)[urow] + U * np.abs(v)
+            ub, bub = read('ubias', urow)
+            v = v + ub
+            b = b + bub + U * np.abs(v)
         v, b = act_bound(v, b, o.act)
         if o.post_s >= 0:
             ps = self.w(o.post_s, o.Cout)[None]
             v = v * ps + self.w(o.post_h, o.Cout)[None]
             b = np.abs(ps) * b + U * np.abs(v)
         if o.gate != L.BUF_NONE:
-            g = self.rd(o.gate, o.B * o.n_seg, o.Cout, 0, o.Cout)[urow]
-            bg = self.rdb(o.gate, o.B * o.n_seg, o.Cout, 0, o.Cout)[urow]
+            g, bg = read('gate', urow)
             b = np.abs(g) * b + np.abs(v) * bg
             v = v * g
             b = b + U * np.abs(v)
         if o.res != L.BUF_NONE:
-            v = v + self.rd(o.res, M, o.res_ld, o.res_coff, o.Cout)
-            b = b + self.rdb(o.res, M, o.res_ld, o.res_coff, o.Cout) + U * np.abs(v)
+            r, br = read('res', m)
+            v = v + r
+            b = b + br + U * np.abs(v)
         v, b = act_bound(v, b, o.act2)
-        self.wr(o.dst, M, o.out_ld, o.out_coff, o.Cout, v, b)
+        out = {'dst': (v, b + stored(v))}                       # + the fp32 store's rounding
         if o.sum != L.BUF_NONE:
-            sv = self.rd(o.sum, M, o.sum_ld, o.sum_coff, o.Cout) + v
-            sb = self.rdb(o.sum, M, o.sum_ld, o.sum_coff, o.Cout) + b + U * np.abs(sv)
-            self.wr(o.sum, M, o.sum_ld, o.sum_coff, o.Cout, sv, sb)
+            sv, sb = read('sum', m)
+            sv = sv + v
+            sb = sb + b + U * np.abs(sv)
+            out['sum'] = (sv, sb + stored(sv))
+        return out
 
     # ---- glue kernels (pool.cu) ----
     @staticmethod
@@ -326,10 +483,10 @@ class BoundSim(Sim):
         pre = np.cumsum(P[:, -1], axis=1)
         return pre[:, -1], bT.sum(1) + chains + U * np.abs(pre[:, 1:]).sum(1)
 
-    def colstats(self, o):
+    def colstats(self, o, read=None):
         R = o.Tin * o.Fin
-        X = self.rd(o.src, o.B * R, o.in_ld, o.in_coff, o.Cin).reshape(o.B, R, o.Cin)
-        bX = self.rdb(o.src, o.B * R, o.in_ld, o.in_coff, o.Cin).reshape(o.B, R, o.Cin)
+        X, bX = (read or self.reader(o))('src', np.arange(o.B * R))
+        X, bX = X.reshape(o.B, R, o.Cin), bX.reshape(o.B, R, o.Cin)
         tot, btot = self._warp_sum(X, bX)
         if o.mode == L.STATS_SEG_CONTEXT:
             segs = [self._warp_sum(X[:, s * o.seg_len:(s + 1) * o.seg_len], bX[:, s * o.seg_len:(s + 1) * o.seg_len])
@@ -347,13 +504,11 @@ class BoundSim(Sim):
                 q = ss / cnt
                 out[:, s] = mean + q
                 bout[:, s] = bmean + bss / cnt + U * np.abs(q) + U * np.abs(out[:, s])
-            self.wr(o.dst, o.B * o.n_seg, o.out_ld, o.out_coff, o.Cin, out.reshape(-1, o.Cin), bout.reshape(-1, o.Cin))
-            return
+            return self._out(o, out.reshape(-1, o.Cin), bout.reshape(-1, o.Cin), read)
         mean = tot / R
         bmean = btot / R + U * np.abs(mean)
         if o.mode == L.STATS_MEAN:
-            self.wr(o.dst, o.B, o.out_ld, o.out_coff, o.Cin, mean, bmean)
-            return
+            return self._out(o, mean, bmean, read)
         d = X - mean[:, None]
         bd = bX + bmean[:, None] + U * np.abs(d)
         ssq, bssq = self._warp_sum(d * d, 2 * np.abs(d) * bd + bd * bd)     # fmaf(d, d, q): the chain's roundings
@@ -371,15 +526,20 @@ class BoundSim(Sim):
                 bt = bt + U * t
             sd = np.sqrt(t)
             bsd = bt / (sd + np.sqrt(np.maximum(t - bt, 0))) + U * sd
-        self.wr(o.dst, o.B, o.out_ld, o.out_coff, 2 * o.Cin, np.concatenate([mean, sd], 1),
-                np.concatenate([bmean, bsd], 1))
+        return self._out(o, np.concatenate([mean, sd], 1), np.concatenate([bmean, bsd], 1), read)
 
-    def asp(self, o):
+    def _out(self, o, v, b, read, exact=False):
+        """{'dst': (v, bound)}, the bound with the fp32 store's rounding unless the op is exact; stored when ``read`` is
+        None (the interpreter's own run)."""
+        out = {'dst': (v, b if exact else b + stored(v))}
+        return self._store(o, out) if read is None else out
+
+    def asp(self, o, read=None):
         T, Cn = o.Tin, o.Cin
-        X = self.rd(o.src, o.B * T, o.in_ld, o.in_coff, Cn).reshape(o.B, T, Cn)
-        bX = self.rdb(o.src, o.B * T, o.in_ld, o.in_coff, Cn).reshape(o.B, T, Cn)
-        Lg = self.rd(o.src2, o.B * T, o.src2_ld, o.src2_coff, Cn).reshape(o.B, T, Cn)
-        bL = self.rdb(o.src2, o.B * T, o.src2_ld, o.src2_coff, Cn).reshape(o.B, T, Cn)
+        rd = read or self.reader(o)
+        X, bX = rd('src', np.arange(o.B * T))
+        Lg, bL = rd('src2', np.arange(o.B * T))
+        X, bX, Lg, bL = (a.reshape(o.B, T, Cn) for a in (X, bX, Lg, bL))
         z = Lg - Lg.max(1, keepdims=True)
         dz = U * np.abs(z) + bL + bL.max(1, keepdims=True)
         e = np.exp(z)
@@ -389,8 +549,7 @@ class BoundSim(Sim):
         mean = sx / se
         bmean = (bsx + np.abs(mean) * bse) / (se - bse) + U * np.abs(mean)
         if o.mode == 1:
-            self.wr(o.dst, o.B, o.out_ld, o.out_coff, Cn, mean, bmean)
-            return
+            return self._out(o, mean, bmean, read)
         d = X - mean[:, None]
         bd = bX + bmean[:, None] + U * np.abs(d)
         dd = d * d
@@ -402,56 +561,50 @@ class BoundSim(Sim):
         t = np.maximum(t, o.eps)
         sd = np.sqrt(t)
         bsd = bt / (sd + np.sqrt(np.maximum(t - bt, 0))) + U * sd
-        self.wr(o.dst, o.B, o.out_ld, o.out_coff, 2 * Cn, np.concatenate([mean, sd], 1), np.concatenate([bmean, bsd], 1))
+        return self._out(o, np.concatenate([mean, sd], 1), np.concatenate([bmean, bsd], 1), read)
 
-    def pool2d(self, o):
-        X = self.rd(o.src, o.B * o.Tin * o.Fin, o.in_ld, o.in_coff, o.Cin).reshape(o.B, o.Tin, o.Fin, o.Cin)
-        bX = self.rdb(o.src, o.B * o.Tin * o.Fin, o.in_ld, o.in_coff, o.Cin).reshape(o.B, o.Tin, o.Fin, o.Cin)
-        out = np.zeros((o.B, o.Tout, o.Fout, o.Cin))
+    def pool2d(self, o, rows=None, read=None):
+        rd = read or self.reader(o)
+        m = np.arange(o.B * o.Tout * o.Fout) if rows is None else np.asarray(rows)
+        out = np.zeros((len(m), o.Cin))
         bout = np.zeros_like(out)
         n = o.KT * o.KF
-        for to in range(o.Tout):
-            for fo in range(o.Fout):
-                t0, f0 = to * o.sT - o.padT, fo * o.sF - o.padF
-                win = X[:, max(t0, 0):min(t0 + o.KT, o.Tin), max(f0, 0):min(f0 + o.KF, o.Fin)]
-                bw = bX[:, max(t0, 0):min(t0 + o.KT, o.Tin), max(f0, 0):min(f0 + o.KF, o.Fin)]
-                if o.mode == 0:
-                    out[:, to, fo] = win.max(axis=(1, 2))
-                    bout[:, to, fo] = bw.max(axis=(1, 2))
-                    continue
-                part = np.cumsum(win.reshape(o.B, -1, o.Cin), axis=1)
-                out[:, to, fo] = part[:, -1] / n
-                # the in-order sum, then x fl(1 / n): two more roundings
-                bout[:, to, fo] = ((bw.reshape(o.B, -1, o.Cin).sum(1) + U * np.abs(part[:, 1:]).sum(1)) / n
-                                   + 2 * U * np.abs(out[:, to, fo]))
-        self.wr(o.dst, o.B * o.Tout * o.Fout, o.out_ld, o.out_coff, o.Cin, out.reshape(-1, o.Cin),
-                bout.reshape(-1, o.Cin), exact=o.mode == 0)
+        for sel, win in pool_windows(o, m):
+            W, bW = (a.reshape(win.shape + (o.Cin,)) for a in rd('src', win.reshape(-1)))
+            if o.mode == 0:
+                out[sel] = W.max(axis=1)
+                bout[sel] = bW.max(axis=1)
+                continue
+            part = np.cumsum(W, axis=1)
+            out[sel] = part[:, -1] / n
+            # the in-order sum, then x fl(1 / n): two more roundings
+            bout[sel] = (bW.sum(1) + U * np.abs(part[:, 1:]).sum(1)) / n + 2 * U * np.abs(out[sel])
+        return self._out(o, out, bout, None if rows is None and read is None else rd, exact=o.mode == 0)
 
-    def ew(self, o):
-        rpu = o.Tin * o.Fin
-        rows = o.B * rpu
-        v = self.rd(o.src, rows, o.in_ld, o.in_coff, o.Cin)
-        b = self.rdb(o.src, rows, o.in_ld, o.in_coff, o.Cin)
+    def ew(self, o, rows=None, read=None):
+        rd = read or self.reader(o)
+        m = np.arange(o.B * o.Tin * o.Fin) if rows is None else np.asarray(rows)
+        keep = None if rows is None and read is None else rd
+        v, b = rd('src', m)
         if o.mode == L.EW_PAD_COPY:
-            self.wr(o.dst, rows, o.out_ld, o.out_coff, o.Cout, np.pad(v, ((0, 0), (0, o.Cout - o.Cin))),
-                    np.pad(b, ((0, 0), (0, o.Cout - o.Cin))), exact=True)
-            return
+            return self._out(o, np.pad(v, ((0, 0), (0, o.Cout - o.Cin))), np.pad(b, ((0, 0), (0, o.Cout - o.Cin))),
+                             keep, exact=True)
         if o.mode == L.EW_GATE_RES:
             if o.gate != L.BUF_NONE:
-                u = np.arange(rows) // rpu
-                g = self.rd(o.gate, o.B, o.Cin, 0, o.Cin)[u]
-                b = np.abs(g) * b + np.abs(v) * self.rdb(o.gate, o.B, o.Cin, 0, o.Cin)[u]
+                g, bg = rd('gate', m // (o.Tin * o.Fin))
+                b = np.abs(g) * b + np.abs(v) * bg
                 v = v * g
                 b = b + U * np.abs(v)
             if o.res != L.BUF_NONE:
-                v = v + self.rd(o.res, rows, o.res_ld, o.res_coff, o.Cin)
-                b = b + self.rdb(o.res, rows, o.res_ld, o.res_coff, o.Cin) + U * np.abs(v)
+                r, br = rd('res', m)
+                v = v + r
+                b = b + br + U * np.abs(v)
             v, b = act_bound(v, b, o.act2)
         elif o.mode == L.EW_AFF:
-            y = self.rd(o.src2, rows, o.src2_ld, o.src2_coff, o.Cin)
-            by = self.rdb(o.src2, rows, o.src2_ld, o.src2_coff, o.Cin)
-            t = np.tanh(self.rd(o.res, rows, o.res_ld, o.res_coff, o.Cin))
-            bt = self.rdb(o.res, rows, o.res_ld, o.res_coff, o.Cin) + 2.0 ** -22 * np.abs(t)
+            y, by = rd('src2', m)
+            att, batt = rd('res', m)
+            t = np.tanh(att)
+            bt = batt + 2.0 ** -22 * np.abs(t)
             a = 1 + t
             ba = bt + U * np.abs(a)
             c = 2 - a
@@ -461,9 +614,18 @@ class BoundSim(Sim):
             v = p1 + p2
             b = b + U * np.abs(v)
         else:                                                     # EW_COPY
-            self.wr(o.dst, rows, o.out_ld, o.out_coff, o.Cin, v, b, exact=True)
-            return
-        self.wr(o.dst, rows, o.out_ld, o.out_coff, o.Cin, v, b)
+            return self._out(o, v, b, keep, exact=True)
+        return self._out(o, v, b, keep)
+
+    def op(self, o, rows=None, read=None, s=None):
+        """Any op: its outputs on ``rows`` (colstats / asp: every row) from the operands ``read`` gives."""
+        if o.kind in (L.OP_CONV, L.OP_CONV_C1):
+            return self.conv(o, rows, read, s)
+        if o.kind == L.OP_EW:
+            return self.ew(o, rows, read)
+        if o.kind == L.OP_POOL2D:
+            return self.pool2d(o, rows, read)
+        return {L.OP_COLSTATS: self.colstats, L.OP_ASP_POOL: self.asp}[o.kind](o, read)
 
 
 _CACHE = {}

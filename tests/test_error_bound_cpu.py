@@ -116,7 +116,7 @@ class Gemm:
         s = eb.BoundSim(b.pb, b.blob, b.X)
         for s.i, op in enumerate(b.pb.ops[:b.main]):               # the copies that feed the op
             {L.OP_EW: s.ew}[op.kind](op)
-        X, _ = s._operand(o)
+        X, _ = s._operand(o, s.reader(o), np.arange(o.B * o.Tin * o.Fin))
         M = o.B * o.Tout * o.Fout
         self.m = np.arange(max(0, M - rows), M)
         self.A, _ = s._im2col(X, np.zeros_like(X), o, self.m)
