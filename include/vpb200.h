@@ -6,10 +6,10 @@
  *     seam 2  predictor(features) -> [B, embd_dim]                          mvector/predict.py:228,262
  * driven by MVectorPredictor.predict / predict_batch (mvector/predict.py:214-265).  This header is the C ABI a
  * maintainer binds (ctypes stub in INTEGRATION.md) to replace exactly those two callables:
- *     vp_fbank / vp_melspec   <-> seam 1 (KaldiFbank: featurizer.py:119-132 -> torchaudio kaldi.py:514-645;
+ *     vp_features             <-> seam 1 (KaldiFbank: featurizer.py:119-132 -> torchaudio kaldi.py:514-645;
  *                                          MelSpectrogram: featurizer.py:41-42,76; CMN + mask: featurizer.py:77-90)
  *     vp_embed                <-> seam 2 (nn.Sequential(build_model(...)).eval(), predict.py:54-63)
- *     vp_embed_wave           <-> seam 1 + seam 2 back to back (predict.py:256-262)
+ *     vp_features + vp_embed  <-> seam 1 + seam 2 back to back (predict.py:256-262)
  *
  * Conventions: all tensor arguments are caller-owned DEVICE pointers to float32 (row-major, dense); every call
  * takes the CUDA stream to enqueue on (a cudaStream_t passed as void*, NULL = legacy default stream) and is
@@ -29,7 +29,7 @@
 extern "C" {
 #endif
 
-#define VP_ABI_VERSION 4
+#define VP_ABI_VERSION 5
 
 enum {
   VP_OK = 0,
@@ -108,25 +108,22 @@ int32_t vp_feature_dim(const vp_handle* h);
 /* number of frames T the configured front-end yields for n_samples (kaldi.py:63-83 / torch.stft; see the framing above) */
 int32_t vp_num_frames(const vp_handle* h, int32_t n_samples);
 
-/* wave [B, Lpad] (zero padded to the batch max, predict.py:248-254) -> feats [B, T, F], T = vp_num_frames(Lpad).
- * keep_frames: device int32 [B] = round(len_i / Lmax * T) (featurizer.py:82-84) or NULL for no masking.
- * scratch: device floats, at least vp_frontend_scratch_floats(B, Lpad).
- * vp_fbank   = torchaudio.compliance.kaldi.fbank per utterance (featurizer.py:47-48,119-132): kind 0, post 0.
- * vp_melspec = torchaudio.transforms.MelSpectrogram, and Spectrogram with a pass-through bank (featurizer.py:41-44):
- *              kind 1, post 0.
- * vp_mfcc    = torchaudio.transforms.MFCC (featurizer.py:45-46): kind 1, post 1.  The top_db clamp uses the maximum
- *              over ALL B utterances of the call, as torchaudio does for a [B, n_mels, T] input. */
+/* The configured front-end: wave [B, Lpad] (zero padded to the batch max, predict.py:248-254) -> feats [B, T, F],
+ * T = vp_num_frames(Lpad).  keep_frames: device int32 [B] = round(len_i / Lmax * T) (featurizer.py:82-84) or NULL
+ * for no masking.  scratch: device floats, at least vp_frontend_scratch_floats(B, Lpad).  What vp_frontend_set
+ * configured decides which torchaudio call this is:
+ *   kind 0, post 0: torchaudio.compliance.kaldi.fbank per utterance (featurizer.py:47-48,119-132);
+ *   kind 1, post 0: torchaudio.transforms.MelSpectrogram, and Spectrogram with a pass-through bank
+ *                   (featurizer.py:41-44);
+ *   kind 1, post 1: torchaudio.transforms.MFCC (featurizer.py:45-46).  The top_db clamp uses the maximum over ALL B
+ *                   utterances of the call, as torchaudio does for a [B, n_mels, T] input. */
 size_t vp_frontend_scratch_floats(const vp_handle* h, int32_t B, int32_t Lpad);
-int vp_fbank(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep_frames, float* feats,
-             float* scratch, void* stream);
-int vp_melspec(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep_frames, float* feats,
-               float* scratch, void* stream);
-int vp_mfcc(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep_frames, float* feats,
-            float* scratch, void* stream);
+int vp_features(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep_frames, float* feats,
+                float* scratch, void* stream);
 
-/* The configured front-end (vp_fbank, vp_melspec or vp_mfcc, whichever vp_frontend_set chose) on a ragged batch, every
- * row as if it were the whole call: the reference's eval / feature-extraction mode (reader.py:82-107), which featurizes
- * each file alone and zero-pads the features to the batch's longest (collate_fn.py:5-24).
+/* The configured front-end on a ragged batch, every row as if it were the whole call: the reference's eval /
+ * feature-extraction mode (reader.py:82-107), which featurizes each file alone and zero-pads the features to the batch's
+ * longest (collate_fn.py:5-24).
  *   wave  [B, ld] device floats, row b holding lens[b] samples (lens: device int32 [B], each in [0, ld])
  *   T     the frames of the longest row, vp_num_frames(max lens[b]); 1 <= T <= vp_num_frames(ld)
  *   feats [B, T, F]: row b's first T_b = vp_num_frames(lens[b]) frames are exactly what a one-row call on its lens[b]
@@ -138,19 +135,20 @@ int vp_mfcc(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int3
 int vp_features_each(vp_handle* h, const float* wave, int32_t B, int32_t ld, const int32_t* lens, int32_t T, float* feats,
                      float* scratch, void* stream);
 
-/* vp_mfcc in two stages, for callers that split ONE reference call over several processes (utterance sharding,
- * SURVEY.md 8e): the top_db clamp of torchaudio's MFCC uses the maximum over the WHOLE call, so a sharded call computes
+/* vp_features of the MFCC front-end in two stages, for callers that split ONE reference call over several processes
+ * (utterance sharding, SURVEY.md 8e): the top_db clamp of torchaudio's MFCC uses the maximum over the WHOLE call, so a
+ * sharded call computes
  *   vp_mfcc_mel    : mel dB values of its shard into `scratch`, their maximum into max_out[0] (device float),
  *   (caller)       : all-reduce(MAX) of that one scalar over the ranks (ncclAllReduce / torch.distributed),
  *   vp_mfcc_finish : clamp to max_in[0] - top_db, DCT-II, CMN, mask -> feats.
  * `scratch` (vp_frontend_scratch_floats(B, Lpad) floats) must be left untouched between the two calls.
- * vp_mfcc == vp_mfcc_mel + vp_mfcc_finish with max_in = max_out. */
+ * vp_features == vp_mfcc_mel + vp_mfcc_finish with max_in = max_out. */
 int vp_mfcc_mel(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, float* scratch, float* max_out, void* stream);
 int vp_mfcc_finish(vp_handle* h, int32_t B, int32_t Lpad, const int32_t* keep_frames, float* feats, float* scratch,
                    const float* max_in, void* stream);
 
 /* Host only (no launch, no device access): how a call on B rows of Lpad samples runs frontend_kernel.  stage: 0 for a
- * vp_fbank / vp_melspec call, 1 for the mel stage of vp_mfcc (it must match the configured front-end).  info[8] =
+ * vp_features call, 1 for the MFCC mel stage (it must match the configured front-end).  info[8] =
  *   [0] instantiation: the n_fft of the register-resident kernel (256, 512, 1024, 2048), 0 for the plan-driven one
  *   [1] G, threads per FFT group       [2] tpc, 16-frame tiles per CTA   [3] 1 when the CTA caches its features on chip
  *   [4] FFT passes                     [5] mel projection: 0 plain loop, 1 four interleaved chains
@@ -248,8 +246,8 @@ typedef struct vp_op {
 } vp_op;
 
 /* Upload the packed fp32 weight arena (host pointer, copied to the device; replaces any previous arena).  Programs
- * created before the call -- whether it succeeds or not -- are validated against the old arena: vp_embed,
- * vp_embed_profiled and vp_embed_wave refuse them with VP_ERR_INVALID before launching anything. */
+ * created before the call -- whether it succeeds or not -- are validated against the old arena: vp_embed and
+ * vp_embed_profiled refuse them with VP_ERR_INVALID before launching anything. */
 int vp_weights_load(vp_handle* h, const void* host_blob, size_t nbytes);
 
 /* Validate + own a program for fixed (B, T).  Its workspace is the handle's shared arena, grown (after draining the
@@ -260,9 +258,6 @@ int vp_program_create(vp_handle* h, const vp_op* ops, int32_t n_ops, size_t work
 void vp_program_destroy(vp_program* p);
 /* feats [B,T,F] -> emb [B, embd_dim] */
 int vp_embed(vp_program* p, const float* feats, float* emb, void* stream);
-/* wave [B,Lpad] -> emb: front-end then program; feats_scratch holds B*T*F floats, fe_scratch as for vp_fbank */
-int vp_embed_wave(vp_program* p, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep_frames,
-                  float* feats_scratch, float* fe_scratch, float* emb, void* stream);
 /* Same as vp_embed but brackets every op with CUDA events on `stream`, synchronises, and writes the per-op device
  * time in milliseconds to the HOST array ms_per_op[n_ops] (bench.py's live roofline measurement). */
 int vp_embed_profiled(vp_program* p, const float* feats, float* emb, void* stream, float* ms_per_op);

@@ -214,7 +214,7 @@ MEL256 = dict(n_fft=256, hop_length=64)
 # round(len / Lpad * T), as predict's ratios give); gain: per-row amplitude, or a (burst, pause) pair of amplitudes that
 # alternate every `segment` samples; intent: the plan the case is meant to reach.
 CASES = {
-    # ---- Kaldi kind (vp_fbank) ----
+    # ---- Kaldi kind (vp_features, kind 0) ----
     'fbank80_512_tpc1_residues': dict(
         method='Fbank', args=FB80, T=47, extra=3, lens=[1.0, 1.0, 0.8, 0.55],
         intent=dict(inst=512, G=64, tpc=1, cache=1, mel='chain4'),
@@ -268,7 +268,7 @@ CASES = {
         T=64, extra=13, lens=[1.0, 0.5],
         intent=dict(inst=0, G=32, tpc=4, cache=1, mel='plain'),
         why='plan-driven n_fft 200 = 8 5 5 at G = 32: the one-warp frame means on <0>'),
-    # ---- STFT kind (vp_melspec) ----
+    # ---- STFT kind (vp_features, kind 1) ----
     'mel40_256_tpc4_reflect': dict(
         method='MelSpectrogram', args=dict(MEL256, n_mels=40), T=57, extra=5,
         intent=dict(inst=256, G=32, tpc=4, cache=1, mel='chain4'),
@@ -330,7 +330,7 @@ CASES = {
     'spec129_256_tpc2': dict(
         method='Spectrogram', args=dict(n_fft=256, hop_length=64), T=45, extra=3,
         intent=dict(inst=256, G=32, tpc=2, cache=1, mel='chain4'), why='F = 129 > 128 with the cache, tpc 2'),
-    # ---- MFCC (vp_mfcc: the mel stage emits per-CTA maxima) ----
+    # ---- MFCC (vp_features, post 1: the mel stage emits per-CTA maxima) ----
     'mfcc_1024_tpc1': dict(
         method='MFCC', args=dict(melkwargs=dict(n_fft=1024, hop_length=256, n_mels=128)), T=31, extra=0,
         lens=[1.0, 0.6], intent=dict(inst=1024, G=128, tpc=1, cache=0, mel='chain4'),

@@ -121,25 +121,29 @@ def test_program_cache_shares_one_workspace_arena():
     assert max(ws) <= sizes[-1] < sum(ws)
 
 
-def test_embed_wave_rejects_mismatched_call_before_launching():
-    """ADVICE r1: vp_embed_wave must validate (B, Lpad) against the program before the front-end writes anything."""
-    import ctypes as C
-    from mvector import _lib as L
-    c = CASES['c2']
-    pred = _predictor(c, _weights(c, seed=5))
-    fz = pred._audio_featurizer
-    T = fz.num_frames(16000)
-    prog = pred.predictor.program(2, T)
-    wave = torch.zeros(3, 16000, device='cuda')
-    feats = torch.full((2 * T * 80,), 7.0, device='cuda')                    # sized from the PROGRAM (2 utterances)
-    scratch = torch.zeros(int(L.lib().vp_frontend_scratch_floats(fz.engine.handle, 3, 16000)), device='cuda')
-    emb = torch.zeros(2, 192, device='cuda')
-    with pytest.raises(L.VpError):
-        prog.run_wave(wave, None, feats, scratch, emb)                       # B = 3 against a B = 2 program
-    with pytest.raises(L.VpError):
-        prog.run_wave(wave[:2, :8000].contiguous(), None, feats, scratch, emb)   # right B, wrong length
-    torch.cuda.synchronize()
-    assert bool((feats == 7.0).all())                                        # nothing was launched
+@pytest.mark.parametrize('feature', ['Fbank', 'MFCC'])
+def test_embed_device_across_chunks_equals_predict_batch(feature, monkeypatch):
+    """embed_device featurizes the whole batch in one call, then runs one program per chunk: with the batch spread over
+    three chunks its embeddings equal predict_batch's (same chunks) bit for bit, MFCC's call-wide clamp included."""
+    from mvector.predict import MVectorPredictor
+    c = dict(CASES['c2'])
+    c['margs'] = dict(embd_dim=192, pooling_type='ASP', channels=[128, 128, 128, 128, 384], attention_channels=64,
+                      res2net_scale=4, se_channels=32)
+    if feature == 'MFCC':
+        c['feature'], c['fargs'], c['fdim'] = 'MFCC', dict(n_mfcc=40), 40
+    monkeypatch.setattr(MVectorPredictor, 'MAX_BATCH', 4)
+    pred = _predictor(c, _weights(c, seed=11))
+    g = torch.Generator().manual_seed(12)
+    lens = [16000, 48000, 30001, 8000, 21000, 40000, 12000, 48000, 25000, 9000]
+    amp = [0.1, 0.3, 0.1, 0.2, 0.05, 0.1, 0.1, 0.2, 0.1, 1e-4]      # a quiet last row: clamped by the first chunk's max
+    waves = [(torch.randn(n, generator=g) * a).numpy() for n, a in zip(lens, amp)]
+    B, lmax = len(lens), max(lens)
+    assert pred._chunk_size(B, pred._audio_featurizer.num_frames(lmax)) == 4        # chunks of 4, 4 and 2 rows
+    x = np.zeros((B, lmax), dtype=np.float32)
+    for i, w in enumerate(waves):
+        x[i, :w.shape[0]] = w
+    got = pred.embed_device(torch.from_numpy(x).cuda(), lens)
+    assert np.array_equal(got.cpu().numpy(), pred.predict_batch(waves))
 
 
 # ------------------------------------------------------------------------------------------------ sharded product path

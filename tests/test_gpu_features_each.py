@@ -84,7 +84,7 @@ def test_mfcc_rows_clamp_against_their_own_maximum():
     ld = 16000
     rows = [(rng.standard_normal(ld) * a).astype(np.float32) for a in (1e-5, 1.0, 1e-5)]
     got = _check_rows(fz, rows, ld)
-    # Rows of one length frame and mean-normalise the same alone as in one vp_mfcc call over the batch, so the only
+    # Rows of one length frame and mean-normalise the same alone as in one vp_features call over the batch, so the only
     # difference left is the clamp: the batch call clamps every row against the loud row's maximum.
     w = np.zeros((3, ld), dtype=np.float32)
     for i, r in enumerate(rows):
@@ -167,8 +167,8 @@ def test_evaluate_equals_the_per_file_loop(tmp_path, method, args, monkeypatch):
     monkeypatch.setattr(MVectorTrainer, 'MAX_GROUP', 7)          # 6 files a group: several groups
     lib = L.lib()
     calls = []
-    for name in ('vp_flac_decode', 'vp_pcm_decode', 'vp_resample', 'vp_gain_normalize', 'vp_features_each', 'vp_fbank',
-                 'vp_mfcc'):
+    for name in ('vp_flac_decode', 'vp_pcm_decode', 'vp_resample', 'vp_gain_normalize', 'vp_features_each',
+                 'vp_features'):
         real = getattr(lib, name)
         monkeypatch.setattr(lib, name, lambda *a, _n=name, _r=real: calls.append(_n) or _r(*a))
     got, labels = tr._embed_list(lst)
@@ -178,7 +178,7 @@ def test_evaluate_equals_the_per_file_loop(tmp_path, method, args, monkeypatch):
         assert calls.count(name) == groups, (name, calls.count(name))
     for name in ('vp_flac_decode', 'vp_pcm_decode', 'vp_resample'):
         assert 0 < calls.count(name) <= groups, (name, calls.count(name))
-    assert 'vp_fbank' not in calls and 'vp_mfcc' not in calls
+    assert 'vp_features' not in calls
     res = tr.evaluate()
     monkeypatch.setattr(MVectorTrainer, '_embed_list', lambda self, name: (_per_file_embeddings(self, name), labels))
     assert tr.evaluate() == res

@@ -90,9 +90,9 @@ def test_frontend_case(name, engine):
 
 
 def test_mfcc_two_stage_matches_one_stage(engine):
-    """vp_mfcc_mel + vp_mfcc_finish (the sharded MFCC's two halves, here on one process) are bit-identical to vp_mfcc on
-    the case with 320 per-CTA maxima whose largest sits at index >= 304: max_reduce_kernel must read past its first
-    256."""
+    """vp_mfcc_mel + vp_mfcc_finish (the sharded MFCC's two halves, here on one process) are bit-identical to
+    vp_features on the case with 320 per-CTA maxima whose largest sits at index >= 304: max_reduce_kernel must read past
+    its first 256."""
     name = fc.TWO_STAGE
     c = fc.CASES[name]
     x, _, _, T = fc.materialize(name)

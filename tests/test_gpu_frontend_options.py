@@ -105,8 +105,8 @@ def test_frontend_set_restores_the_default_framing():
     wd = x.cuda().contiguous()
     feats = torch.empty(B, T, 64, device='cuda')
     scratch = torch.empty(int(lib.vp_frontend_scratch_floats(h, B, Lp)), device='cuda')
-    check(h, lib.vp_melspec(h, C.c_void_p(wd.data_ptr()), B, Lp, None, C.c_void_p(feats.data_ptr()),
-                            C.c_void_p(scratch.data_ptr()), fz.engine.stream_ptr()))
+    check(h, lib.vp_features(h, C.c_void_p(wd.data_ptr()), B, Lp, None, C.c_void_p(feats.data_ptr()),
+                             C.c_void_p(scratch.data_ptr()), fz.engine.stream_ptr()))
     torch.cuda.synchronize()
     assert torch.equal(feats.cpu(), _fz('MelSpectrogram', args)(x).cpu())
 
@@ -121,9 +121,15 @@ def test_two_stage_mfcc_honours_the_options():
     B, Lp = w.shape
     keep = fz.keep_frames(ratio, fz.num_frames(Lp)).cuda()
     from mvector import _lib as L
+    from mvector.engine import _check as check
+    lib, h, st = L.lib(), fz.engine.handle, fz.engine.stream_ptr()
     feats = torch.empty_like(one_call)
-    scratch = torch.empty(int(L.lib().vp_frontend_scratch_floats(fz.engine.handle, B, Lp)), device='cuda')
-    fz.mfcc_sharded(w, B, Lp, C.c_void_p(keep.data_ptr()), feats, scratch, torch.cuda.current_stream(), None)
+    scratch = torch.empty(int(lib.vp_frontend_scratch_floats(h, B, Lp)), device='cuda')
+    mx = torch.empty(1, device='cuda')
+    check(h, lib.vp_mfcc_mel(h, C.c_void_p(w.data_ptr()), B, Lp, C.c_void_p(scratch.data_ptr()),
+                             C.c_void_p(mx.data_ptr()), st))
+    check(h, lib.vp_mfcc_finish(h, B, Lp, C.c_void_p(keep.data_ptr()), C.c_void_p(feats.data_ptr()),
+                                C.c_void_p(scratch.data_ptr()), C.c_void_p(mx.data_ptr()), st))
     torch.cuda.synchronize()
     assert torch.equal(feats, one_call)
 

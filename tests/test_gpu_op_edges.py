@@ -280,10 +280,9 @@ def test_graph_recaptured_after_arena_growth():
 
 
 def test_programs_refused_after_weight_reload():
-    """A program validated against one weights blob is refused once another is loaded -- run, run_profiled and
-    run_wave raise VP_ERR_INVALID before anything is launched (the output stays NaN) -- rather than replay a graph
-    that reads the freed blob with the old blob's offsets and fp16 descales.  A program created after the reload runs
-    on the new blob."""
+    """A program validated against one weights blob is refused once another is loaded -- run and run_profiled raise
+    VP_ERR_INVALID before anything is launched (the output stays NaN) -- rather than replay a graph that reads the freed
+    blob with the old blob's offsets and fp16 descales.  A program created after the reload runs on the new blob."""
     from mvector.engine import Engine, Program
     old, new = oc.build(LIFECYCLE), oc.build(dict(oc.GRAPH_RESET))
     assert new.blob.nbytes < old.blob.nbytes                          # the old offsets would overrun the new blob
@@ -295,9 +294,7 @@ def test_programs_refused_after_weight_reload():
         _graphed(prog, x, y)
         _graphed(prog, x, y)                                           # captured
         eng.load_weights(new.blob)
-        wave = torch.zeros(4, 16000, device='cuda')
-        for what, call in (('run', lambda: prog.run(x, y)), ('run_profiled', lambda: prog.run_profiled(x, y)),
-                           ('run_wave', lambda: prog.run_wave(wave, None, x, x, y))):
+        for what, call in (('run', lambda: prog.run(x, y)), ('run_profiled', lambda: prog.run_profiled(x, y))):
             y.fill_(float('nan'))
             with pytest.raises(L.VpError) as e:
                 call()

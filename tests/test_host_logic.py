@@ -25,7 +25,7 @@ def test_cabi_library_exports_every_declared_symbol():
     from mvector import _lib
     assert set(_lib.EXPORTS) == declared
     L = _lib.lib()
-    assert L.vp_abi_version() == 4
+    assert L.vp_abi_version() == 5
     assert L.vp_sizeof_op() == ctypes.sizeof(_lib.Op)
 
 

@@ -26,7 +26,7 @@ def export(model, B, T, path):
     ops = (L.Op * len(pb.ops))(*pb.ops)
     with open(path, 'wb') as f:
         f.write(MAGIC)
-        f.write(struct.pack('<8i', 4, C.sizeof(L.Op), len(pb.ops), B, T, model.input_size, model.embd_dim, 0))
+        f.write(struct.pack('<8i', L.ABI_VERSION, C.sizeof(L.Op), len(pb.ops), B, T, model.input_size, model.embd_dim, 0))
         f.write(struct.pack('<4Q', max(pb.peak, 256), pb.in_floats, pb.out_floats, blob.nbytes))
         f.write(bytes(ops))
         f.write(blob.tobytes())

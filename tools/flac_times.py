@@ -1,7 +1,7 @@
 """FLAC decoding on the device (csrc/flac.cu): kernel time of vp_flac_decode on 256 x 3 s 16 kHz mono and 256 x 3 s
 44.1 kHz stereo (CUDA events over many launches; one 3 s stream written by the test encoder, FIXED order 2 with Rice
 partitions, repeated 256 times), with the compressed bytes in and samples out; beside it the front-end of the same
-256 x 3 s 16 kHz batch (vp_fbank), and predict_batch end to end from the FLAC bytes against the same audio as float32
+256 x 3 s 16 kHz batch (Fbank), and predict_batch end to end from the FLAC bytes against the same audio as float32
 arrays, outputs compared; one hour at 16 kHz in one stream (a 10 s encoded chunk's frames repeated under new frame
 numbers); evaluate over 64 synthetic 3 s files as FLAC and as 16-bit WAV, results compared.
 

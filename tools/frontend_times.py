@@ -5,10 +5,11 @@
 
 Loads the base checkout's package and library, and this tree's, in turn (one process each, VPB_LIB naming the library,
 alternating for --rounds rounds) on the same seeded 256 x 3 s batch: checks that Fbank-80, MelSpectrogram-64,
-Spectrogram-400 and MFCC features are bit-identical between the two, and times vp_fbank at that shape with CUDA events after a warm-up,
-and beside it, through AudioFeaturizer, MelSpectrogram-64 (n_fft 1024) at 128 x 5 s and Spectrogram-400 (the mixed-radix
-FFT path) at 256 x 3 s.  Then times every framing option of this tree's library at the 256 x 3 s shape.  Prints the card's
-name and power limit with the numbers.
+Spectrogram-400 and MFCC features are bit-identical between the two, and times the Fbank call (vp_features: the base
+needs ABI v5 or later) at that shape with CUDA events after a warm-up, and beside it, through AudioFeaturizer,
+MelSpectrogram-64 (n_fft 1024) at 128 x 5 s and Spectrogram-400 (the mixed-radix FFT path) at 256 x 3 s.  Then times
+every framing option of this tree's library at the 256 x 3 s shape.  Prints the card's name and power limit with the
+numbers.
 """
 import argparse
 import ctypes as C
@@ -81,9 +82,9 @@ def child(root, out, modes):
     y = torch.empty(B, T, 80, device='cuda')
     scratch = torch.empty(int(lib.vp_frontend_scratch_floats(h, B, N)), device='cuda')
     sp = fz.engine.stream_ptr()
-    res['vp_fbank_ms'] = _time(lambda: _check(h, lib.vp_fbank(h, C.c_void_p(w.data_ptr()), B, N, None,
-                                                              C.c_void_p(y.data_ptr()), C.c_void_p(scratch.data_ptr()),
-                                                              sp)))
+    res['fbank_ms'] = _time(lambda: _check(h, lib.vp_features(h, C.c_void_p(w.data_ptr()), B, N, None,
+                                                           C.c_void_p(y.data_ptr()), C.c_void_p(scratch.data_ptr()),
+                                                           sp)))
     w5 = (torch.randn(128, 80000, generator=torch.Generator().manual_seed(1)) * 0.1).cuda()
     mel, spec = AudioFeaturizer('MelSpectrogram', method_args=CONFIGS[1][1]), AudioFeaturizer('Spectrogram', method_args={})
     res['beside_ms'] = {'MelSpectrogram-64 n_fft 1024, 128 x 80000': _time(lambda: mel(w5)),
@@ -126,7 +127,7 @@ def main():
             with open(o + '.json') as fh:
                 res = json.load(fh)
             assert os.path.samefile(res['lib'], path) and res['package'].startswith(root + os.sep), res
-            times[k].append(res['vp_fbank_ms'])
+            times[k].append(res['fbank_ms'])
             for name, t in res['beside_ms'].items():
                 beside[k].setdefault(name, []).append(t)
             modes = res.get('modes', modes)
@@ -139,7 +140,7 @@ def main():
         print(f'{method:15s} {fa[method].shape} bit-identical: {same}')
         assert same, method
     for k in roots:
-        print(f'vp_fbank {B} x {N} samples, {k:4s}: ' + ', '.join(f'{t:.3f}' for t in times[k]) + ' ms')
+        print(f'Fbank call {B} x {N} samples, {k:4s}: ' + ', '.join(f'{t:.3f}' for t in times[k]) + ' ms')
     for k in roots:
         for name, ts in beside[k].items():
             print(f'{name}, {k:4s}: ' + ', '.join(f'{t:.3f}' for t in ts) + ' ms')

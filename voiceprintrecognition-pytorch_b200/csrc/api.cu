@@ -274,17 +274,14 @@ static FrontendParams frontend_params(const vp_handle* h, int B, int L, int T = 
   return p;
 }
 
-// want_kind / want_post: -1 = whatever is configured (vp_embed_wave).
 // stage: 0 = the whole front-end; 1 = MFCC mel stage only (maximum -> ext_max[0]); 2 = MFCC clamp/DCT/CMN only, clamping
 // against the externally reduced maximum ext_max[0].
 // lens (device int32 [B]) non-null: a ragged call of T frames, row b featurized alone on its first lens[b] samples.
-static int run_frontend(vp_handle* h, int want_kind, int want_post, const float* wave, int B, int L, const int32_t* keep,
-                        float* feats, float* scratch, cudaStream_t st, int stage = 0, float* ext_max = nullptr,
-                        const int32_t* lens = nullptr, int T_call = -1) {
+static int run_frontend(vp_handle* h, const float* wave, int B, int L, const int32_t* keep, float* feats, float* scratch,
+                        cudaStream_t st, int stage = 0, float* ext_max = nullptr, const int32_t* lens = nullptr,
+                        int T_call = -1) {
   if (!h) return VP_ERR_INVALID;
   if (!h->fe_set) return fail(h, VP_ERR_INVALID, "front-end not configured (vp_frontend_set)");
-  if (want_kind >= 0 && h->fe.kind != want_kind) return fail(h, VP_ERR_INVALID, "front-end kind mismatch");
-  if (want_post >= 0 && h->fe.post != want_post) return fail(h, VP_ERR_INVALID, "front-end post-stage mismatch (vp_melspec vs vp_mfcc)");
   if ((stage != 2 && !wave) || (stage != 1 && !feats) || !scratch || B < 1) return fail(h, VP_ERR_INVALID, "null/empty argument");
   if (stage != 0 && (h->fe.post != 1 || !ext_max)) return fail(h, VP_ERR_INVALID, "two-stage calls are for the MFCC front-end");
   const char* len_err = frontend_call_error(h, B, L);
@@ -339,31 +336,23 @@ int vp_frontend_plan_info(const vp_handle* h, int32_t B, int32_t Lpad, int32_t s
   return VP_OK;
 }
 
-int vp_fbank(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep, float* feats,
-             float* scratch, void* stream) {
-  return run_frontend(h, 0, 0, wave, B, Lpad, keep, feats, scratch, (cudaStream_t)stream);
-}
-int vp_melspec(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep, float* feats,
-               float* scratch, void* stream) {
-  return run_frontend(h, 1, 0, wave, B, Lpad, keep, feats, scratch, (cudaStream_t)stream);
-}
-int vp_mfcc(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep, float* feats,
-            float* scratch, void* stream) {
-  return run_frontend(h, 1, 1, wave, B, Lpad, keep, feats, scratch, (cudaStream_t)stream);
+int vp_features(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep, float* feats,
+                float* scratch, void* stream) {
+  return run_frontend(h, wave, B, Lpad, keep, feats, scratch, (cudaStream_t)stream);
 }
 
 int vp_features_each(vp_handle* h, const float* wave, int32_t B, int32_t ld, const int32_t* lens, int32_t T, float* feats,
                      float* scratch, void* stream) {
   if (!lens) return fail(h, VP_ERR_INVALID, "null argument");
-  return run_frontend(h, -1, -1, wave, B, ld, nullptr, feats, scratch, (cudaStream_t)stream, 0, nullptr, lens, T);
+  return run_frontend(h, wave, B, ld, nullptr, feats, scratch, (cudaStream_t)stream, 0, nullptr, lens, T);
 }
 
 int vp_mfcc_mel(vp_handle* h, const float* wave, int32_t B, int32_t Lpad, float* scratch, float* max_out, void* stream) {
-  return run_frontend(h, 1, 1, wave, B, Lpad, nullptr, nullptr, scratch, (cudaStream_t)stream, 1, max_out);
+  return run_frontend(h, wave, B, Lpad, nullptr, nullptr, scratch, (cudaStream_t)stream, 1, max_out);
 }
 int vp_mfcc_finish(vp_handle* h, int32_t B, int32_t Lpad, const int32_t* keep, float* feats, float* scratch,
                    const float* max_in, void* stream) {
-  return run_frontend(h, 1, 1, nullptr, B, Lpad, keep, feats, scratch, (cudaStream_t)stream, 2, const_cast<float*>(max_in));
+  return run_frontend(h, nullptr, B, Lpad, keep, feats, scratch, (cudaStream_t)stream, 2, const_cast<float*>(max_in));
 }
 
 int vp_weights_load(vp_handle* h, const void* blob, size_t nbytes) {
@@ -830,24 +819,6 @@ int vp_program_op_info(const vp_program* p, int32_t i, int32_t* kind, int64_t* M
     *M = (int64_t)o.B * o.Tin * o.Fin; *N = o.Cin; *K = 0;
   }
   return VP_OK;
-}
-
-int vp_embed_wave(vp_program* p, const float* wave, int32_t B, int32_t Lpad, const int32_t* keep, float* feats_scratch,
-                  float* fe_scratch, float* emb, void* stream) {
-  if (!p) return VP_ERR_INVALID;
-  // check the call against the program BEFORE anything is launched: the front-end writes B*T*F floats into
-  // feats_scratch, which a host sizes from the program
-  TRY(check_weights_gen(p));
-  if (!p->h->fe_set) return fail(p->h, VP_ERR_INVALID, "front-end not configured (vp_frontend_set)");
-  const int T = vp_num_frames(p->h, Lpad);
-  if (B < 1 || T < 1) return fail(p->h, VP_ERR_INVALID, "empty batch / waveform shorter than one frame");
-  const size_t need = (size_t)B * T * vp_feature_dim(p->h);
-  if (need != p->in_floats)
-    return fail(p->h, VP_ERR_INVALID, "program expects %zu input floats, the front-end would produce %zu", p->in_floats, need);
-  if (B != p->B) return fail(p->h, VP_ERR_INVALID, "program was lowered for B=%d, called with B=%d", p->B, B);
-  int r = run_frontend(p->h, -1, -1, wave, B, Lpad, keep, feats_scratch, fe_scratch, (cudaStream_t)stream);
-  if (r != VP_OK) return r;
-  return vp_embed(p, feats_scratch, emb, stream);
 }
 
 int vp_device_zero(void* device_ptr, size_t nbytes, void* stream) {

@@ -46,8 +46,8 @@
 // Every butterfly, twiddle product, power and mel sum is the same expression on the same operands in both
 // instantiations, so the features do not depend on which one ran.
 // Bound (DESIGN.md section 4 has the counts): at 256 x 3 s, 73 MB of HBM traffic, ~1 GFLOP of fp64 and ~3.2 GB through
-// shared memory per call.  frontend_kernel<512> takes 0.285 ms there and vp_fbank, with cmn_mask_kernel, 0.307 ms (one
-// H100 80GB HBM3, 700 W; vp_fbank took 0.61 ms before the layouts above): shared memory is the nearest bound, ~3x
+// shared memory per call.  frontend_kernel<512> takes 0.285 ms there and the Fbank call, with cmn_mask_kernel, 0.307 ms
+// (one H100 80GB HBM3, 700 W; the call took 0.61 ms before the layouts above): shared memory is the nearest bound, ~3x
 // away; the rest is barrier and shared-memory latency at the 16 warps per SM that 128 registers allow.
 #include "kernels.cuh"
 

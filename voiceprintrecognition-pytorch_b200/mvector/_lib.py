@@ -6,6 +6,7 @@ import os
 _HERE = os.path.dirname(os.path.abspath(__file__))
 LIB_PATH = os.environ.get('VPB_LIB') or os.path.join(os.path.dirname(_HERE), 'libvpb200.so')   # VPB_LIB: dev builds
 
+ABI_VERSION = 5                 # VP_ABI_VERSION of include/vpb200.h
 VP_OK, VP_ERR_INVALID, VP_ERR_CUDA, VP_ERR_NOMEM, VP_ERR_UNSUPPORTED = 0, 1, 2, 3, 4
 OP_CONV, OP_CONV_C1, OP_COLSTATS, OP_ASP_POOL, OP_EW, OP_POOL2D = 1, 2, 3, 4, 5, 6
 POOL_MAX, POOL_AVG = 0, 1
@@ -98,9 +99,7 @@ def lib():
         'vp_feature_dim': (i32, [vp]),
         'vp_num_frames': (i32, [vp, i32]),
         'vp_frontend_scratch_floats': (sz, [vp, i32, i32]),
-        'vp_fbank': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
-        'vp_melspec': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
-        'vp_mfcc': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
+        'vp_features': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, vp]),
         'vp_features_each': (C.c_int, [vp, f32p, i32, i32, i32p, i32, f32p, f32p, vp]),
         'vp_mfcc_mel': (C.c_int, [vp, f32p, i32, i32, f32p, f32p, vp]),
         'vp_mfcc_finish': (C.c_int, [vp, i32, i32, i32p, f32p, f32p, f32p, vp]),
@@ -109,7 +108,6 @@ def lib():
         'vp_program_create': (C.c_int, [vp, C.POINTER(Op), i32, sz, sz, sz, pp]),
         'vp_program_destroy': (None, [vp]),
         'vp_embed': (C.c_int, [vp, f32p, f32p, vp]),
-        'vp_embed_wave': (C.c_int, [vp, f32p, i32, i32, i32p, f32p, f32p, f32p, vp]),
         'vp_program_launches': (i32, [vp]),
         'vp_embed_profiled': (C.c_int, [vp, f32p, f32p, vp, C.c_void_p]),
         'vp_program_op_info': (C.c_int, [vp, i32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]),
@@ -146,7 +144,7 @@ def lib():
         fn = getattr(L, name)          # AttributeError here = header/library mismatch
         fn.restype = res
         fn.argtypes = args
-    if L.vp_abi_version() != 4:
+    if L.vp_abi_version() != ABI_VERSION:
         raise RuntimeError('libvpb200.so ABI version mismatch')
     if L.vp_sizeof_op() != C.sizeof(Op) or L.vp_sizeof_frontend_desc() != C.sizeof(FrontendDesc) \
             or L.vp_sizeof_frontend_options() != C.sizeof(FrontendOptions) or L.vp_sizeof_flac_info() != C.sizeof(FlacInfo) \
@@ -159,9 +157,9 @@ def lib():
 
 
 EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_create', 'vp_destroy', 'vp_last_error',
-           'vp_frontend_set', 'vp_sizeof_frontend_options', 'vp_frontend_set_options', 'vp_num_frames', 'vp_frontend_scratch_floats', 'vp_fbank', 'vp_melspec', 'vp_mfcc',
+           'vp_frontend_set', 'vp_sizeof_frontend_options', 'vp_frontend_set_options', 'vp_num_frames', 'vp_frontend_scratch_floats', 'vp_features',
            'vp_feature_dim',
-           'vp_weights_load', 'vp_program_create', 'vp_program_destroy', 'vp_embed', 'vp_embed_wave',
+           'vp_weights_load', 'vp_program_create', 'vp_program_destroy', 'vp_embed',
            'vp_program_launches', 'vp_program_peek', 'vp_embed_profiled', 'vp_program_op_info', 'vp_host_gather_pad',
            'vp_host_stage_h2d', 'vp_host_gather_streaming', 'vp_workspace_bytes', 'vp_mfcc_mel', 'vp_mfcc_finish', 'vp_features_each', 'vp_frontend_plan_info', 'vp_cosine_scores', 'vp_device_zero',
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',

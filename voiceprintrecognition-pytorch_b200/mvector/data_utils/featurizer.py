@@ -1,7 +1,7 @@
 """AudioFeaturizer mirror (reference: mvector/data_utils/featurizer.py:9-132), backed by the fused sm_90a front-end.
 
 Host side only prepares constants once (window, sparse mel bank, DCT matrix -- the reference rebuilds the Kaldi ones on
-every call, kaldi.py:201,621-627) and hands device pointers to ``vp_fbank`` / ``vp_melspec`` / ``vp_mfcc``; the
+every call, kaldi.py:201,621-627) and hands device pointers to ``vp_features`` (``AudioFeaturizer.launch``); the
 per-utterance Python loop (featurizer.py:124-131), the transpose, the CMN and the length mask (featurizer.py:77-90) all
 run in two kernels (three for MFCC).  All four ``feature_method`` values of the reference are lowered: Fbank,
 MelSpectrogram, Spectrogram (pass-through bank over the n_fft/2+1 bins) and MFCC.
@@ -399,6 +399,7 @@ class AudioFeaturizer:
             self.feat_fun = MFCC(**method_args)
         else:
             raise Exception(f'预处理方法 {self._feature_method} 不存在!')
+        self.whole_call = self.feat_fun.desc.post == 1 and self.feat_fun.desc.top_db >= 0    # MFCC's call-wide clamp
         self._engine = engine
         self._configured = False
         logger.info(f'使用【{feature_method}】提取特征')
@@ -439,6 +440,13 @@ class AudioFeaturizer:
             return 0 if n < f.n_fft else 1 + (n - f.n_fft) // f.hop
         return 1 + n // f.hop
 
+    def call_frames(self, n_samples):
+        """num_frames of a padded call, which refuses a Kaldi window longer than its rows as the reference does."""
+        f = self.feat_fun
+        if f.desc.kind == 0:                            # kaldi.py:141
+            assert 2 <= f.win_length <= n_samples, f'choose a window size {f.win_length} that is [2, {n_samples}]'
+        return self.num_frames(n_samples)
+
     @staticmethod
     def keep_frames(input_lens_ratio, T):
         """featurizer.py:82-84: mask_lens = round(ratio * T) in float32, half-to-even."""
@@ -467,26 +475,40 @@ class AudioFeaturizer:
     def forward_keep(self, w, keep=None, group=None):
         """Same with the mask lengths already on the device: ``w`` CUDA float32 [B, L] contiguous, ``keep`` CUDA int32 [B]
         (frames kept per utterance, featurizer.py:82-84) or None."""
-        self._ensure()
-        dev = self._engine.device
         B, Lp = w.shape
-        f = self.feat_fun
-        if f.desc.kind == 0:
-            assert 2 <= f.win_length <= Lp, f'choose a window size {f.win_length} that is [2, {Lp}]'
-        T = self.num_frames(Lp)
-        feats = torch.empty(B, T, self.feature_dim, dtype=torch.float32, device=dev)
-        lib = L.lib()
-        scratch = torch.empty(max(int(lib.vp_frontend_scratch_floats(self._engine.handle, B, Lp)), 1),
-                              dtype=torch.float32, device=dev)
-        kp = C.c_void_p(keep.data_ptr()) if keep is not None else C.c_void_p()
-        if group is not None and f.desc.post == 1 and f.desc.top_db >= 0:
-            self.mfcc_sharded(w, B, Lp, kp, feats, scratch, torch.cuda.current_stream(dev), group)
-            return feats
-        fn = lib.vp_fbank if f.desc.kind == 0 else (lib.vp_mfcc if f.desc.post == 1 else lib.vp_melspec)
-        _check(self._engine.handle, fn(self._engine.handle, C.c_void_p(w.data_ptr()), B, Lp, kp,
-                                       C.c_void_p(feats.data_ptr()), C.c_void_p(scratch.data_ptr()),
-                                       self._engine.stream_ptr()))
+        feats = torch.empty(B, self.num_frames(Lp), self.feature_dim, dtype=torch.float32, device=w.device)
+        self.launch(w, feats, torch.cuda.current_stream(w.device), keep, group)
         return feats
+
+    def launch(self, w, feats, stream, keep=None, group=None):
+        """Enqueue vp_features on ``stream`` into ``feats``, a contiguous view of B * T * F floats (``w``, ``keep`` as for
+        forward_keep).  ``group`` shards ONE call by utterances: MFCC then all-reduces (MAX) its clamp maximum between
+        vp_mfcc_mel and vp_mfcc_finish, bit-identical to vp_features on the whole batch."""
+        self._ensure()
+        B, Lp = w.shape
+        assert feats.is_contiguous() and feats.numel() == B * self.call_frames(Lp) * self.feature_dim
+        lib, h = L.lib(), self._engine.handle
+        wp, fp, sp = C.c_void_p(w.data_ptr()), C.c_void_p(feats.data_ptr()), C.c_void_p(stream.cuda_stream)
+        kp = C.c_void_p(keep.data_ptr()) if keep is not None else C.c_void_p()
+        with torch.cuda.stream(stream):
+            scratch = torch.empty(max(int(lib.vp_frontend_scratch_floats(h, B, Lp)), 1), dtype=torch.float32,
+                                  device=w.device)
+            sc = C.c_void_p(scratch.data_ptr())
+            if group is None or not self.whole_call:
+                _check(h, lib.vp_features(h, wp, B, Lp, kp, fp, sc, sp))
+                return
+            import torch.distributed as dist
+            mx = torch.empty(1, dtype=torch.float32, device=w.device)
+            _check(h, lib.vp_mfcc_mel(h, wp, B, Lp, sc, C.c_void_p(mx.data_ptr()), sp))
+            if dist.is_initialized() and dist.get_world_size(group) > 1:
+                from ..distributed import device_collectives
+                if device_collectives(group):
+                    dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=group)
+                else:                                   # gloo: one float through the host
+                    m = mx.cpu()
+                    dist.all_reduce(m, op=dist.ReduceOp.MAX, group=group)
+                    mx.copy_(m)
+            _check(h, lib.vp_mfcc_finish(h, B, Lp, kp, fp, sc, C.c_void_p(mx.data_ptr()), sp))
 
     def forward_each(self, w, lens):
         """Every row of a ragged batch featurized as if it were the whole call (vp_features_each): the reference's
@@ -521,29 +543,6 @@ class AudioFeaturizer:
                                        C.c_void_p(feats.data_ptr()), C.c_void_p(scratch.data_ptr()),
                                        self._engine.stream_ptr()))
         return feats, tb
-
-    def mfcc_sharded(self, w, B, Lp, kp, feats, scratch, stream, group):
-        """MFCC of this rank's shard of ONE sharded call: vp_mfcc_mel -> all-reduce(MAX) of the clamp maximum over
-        ``group`` -> vp_mfcc_finish, all enqueued on ``stream``.  Bit-identical to the single-process vp_mfcc of the whole
-        batch (max is exact and order independent)."""
-        import torch.distributed as dist
-        lib = L.lib()
-        h = self._engine.handle
-        mx = torch.empty(1, dtype=torch.float32, device=feats.device)
-        sp = C.c_void_p(stream.cuda_stream)
-        with torch.cuda.stream(stream):
-            _check(h, lib.vp_mfcc_mel(h, C.c_void_p(w.data_ptr()), B, Lp, C.c_void_p(scratch.data_ptr()),
-                                      C.c_void_p(mx.data_ptr()), sp))
-            if dist.is_initialized() and dist.get_world_size(group) > 1:
-                from ..distributed import device_collectives
-                if device_collectives(group):
-                    dist.all_reduce(mx, op=dist.ReduceOp.MAX, group=group)
-                else:                                   # gloo: one float through the host
-                    m = mx.cpu()
-                    dist.all_reduce(m, op=dist.ReduceOp.MAX, group=group)
-                    mx.copy_(m)
-            _check(h, lib.vp_mfcc_finish(h, B, Lp, kp, C.c_void_p(feats.data_ptr()), C.c_void_p(scratch.data_ptr()),
-                                         C.c_void_p(mx.data_ptr()), sp))
 
     __call__ = forward
 

@@ -796,13 +796,6 @@ class Program:
         _check(self.engine.handle, L.lib().vp_embed(self._p, C.c_void_p(feats.data_ptr()), C.c_void_p(emb.data_ptr()),
                                                     self.engine.stream_ptr()))
 
-    def run_wave(self, wave, keep, feats_scratch, fe_scratch, emb):
-        B, Lpad = wave.shape
-        kp = C.c_void_p(keep.data_ptr()) if keep is not None else C.c_void_p()
-        _check(self.engine.handle, L.lib().vp_embed_wave(
-            self._p, C.c_void_p(wave.data_ptr()), B, Lpad, kp, C.c_void_p(feats_scratch.data_ptr()),
-            C.c_void_p(fe_scratch.data_ptr()), C.c_void_p(emb.data_ptr()), self.engine.stream_ptr()))
-
     def run_profiled(self, feats, emb):
         """vp_embed with per-op CUDA-event timing -> list of dicts (kind, M, N, K, engine, ms)."""
         ms = (C.c_float * self.n_ops)()

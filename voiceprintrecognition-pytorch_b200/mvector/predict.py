@@ -4,7 +4,7 @@ GPU-native path.  Constructor and method signatures, argument meaning and error 
 
 Differences that are deliberate:
   * ``use_gpu=False`` raises: this path has no CPU implementation (the reference's CPU path is the oracle).
-  * ``predict_batch`` feeds the WHOLE padded batch to the device in one ``vp_embed_wave`` call (front-end + backbone);
+  * ``predict_batch`` feeds the WHOLE padded batch to the device (front-end ``vp_features``, backbone ``vp_embed``);
     the reference's ``batch_size`` argument (predict.py:261) is accepted and ignored -- chunking does not change
     results because every op is per-utterance, and padding/CMN/mask are computed on the full batch exactly like
     predict.py:244-258.
@@ -337,10 +337,7 @@ class MVectorPredictor:
         if B == 0:
             e = torch.empty(0, D, dtype=torch.float32, device=dev)
             return e.cpu().numpy() if to_numpy else e
-        T = fz.num_frames(lmax)
-        desc = fz.feat_fun.desc
-        if desc.kind == 0:
-            assert 2 <= fz.feat_fun.win_length <= lmax, f'choose a window size {fz.feat_fun.win_length} that is [2, {lmax}]'
+        T = fz.call_frames(lmax)
         eng = fz.engine
         lib = L.lib()
         F = fz.feature_dim
@@ -359,8 +356,7 @@ class MVectorPredictor:
         emb = torch.empty(B, D, dtype=torch.float32, device=dev)
         feats = torch.empty(B, T * F, dtype=torch.float32, device=dev)
         bounds = np.cumsum(self._host_chunks(B, T)).tolist()       # end row of every backbone chunk
-        whole = desc.post == 1 and desc.top_db >= 0      # MFCC: the top_db clamp needs the maximum over the whole call
-        S = B if whole else min(self.STAGE_ROWS, B)
+        S = B if fz.whole_call else min(self.STAGE_ROWS, B)
         nstages = (B + S - 1) // S
         K = min(nstages, 4)                             # device staging slots (the pinned side always has two)
         dwave = torch.empty(K, S * lmax, dtype=torch.float32, device=dev)
@@ -371,11 +367,9 @@ class MVectorPredictor:
             if plan.gain:
                 flags = torch.empty(B, dtype=torch.int32, device=dev)
                 gscratch = plan.scratch(S, lmax)
-        scratch = torch.empty(max(int(lib.vp_frontend_scratch_floats(eng.handle, S, lmax)), 1), dtype=torch.float32, device=dev)
         cs = self._staging_stream()
         cs_ptr = C.c_void_p(cs.cuda_stream)
         main = torch.cuda.current_stream(dev)
-        main_ptr = C.c_void_p(main.cuda_stream)
         cs.wait_stream(main)                            # buffers handed out by the allocator may still be in use on main
         ptrs = np.empty(B, dtype=np.uint64)              # filled stage by stage: only stage 0's part is on the critical path
         nthreads = self._gather_threads()
@@ -389,7 +383,6 @@ class MVectorPredictor:
                 e.record(stream)
                 dtr.append((label, e))
         dmark('t0 (main stream)', main)
-        fe_fn = lib.vp_fbank if desc.kind == 0 else (lib.vp_mfcc if desc.post == 1 else lib.vp_melspec)
         pin_ev = [None, None]                           # H2D copies out of a pinned slot finished: the host may refill it
         dev_ev = [None] * K                             # front-end finished reading a device slot: the copies may refill it
         next_chunk = 0
@@ -426,13 +419,7 @@ class MVectorPredictor:
             if plan is not None:
                 plan.run(dst, ld, dw, lmax, g0, g1, flags, gscratch, main)
                 dmark(f'stage {gi}: conditioning done', main)
-            kp = C.c_void_p(keep_all.data_ptr() + 4 * g0) if keep_all is not None else C.c_void_p()
-            if whole and group is not None:
-                fz.mfcc_sharded(dw, n, lmax, kp, feats, scratch, main, group)
-            else:
-                from .engine import _check
-                _check(eng.handle, fe_fn(eng.handle, C.c_void_p(dw.data_ptr()), n, lmax, kp,
-                                         C.c_void_p(feats.data_ptr() + 4 * g0 * T * F), C.c_void_p(scratch.data_ptr()), main_ptr))
+            fz.launch(dw[:n * lmax].view(n, lmax), feats[g0:g1], main, None if keep_all is None else keep_all[g0:g1], group)
             fev = torch.cuda.Event()
             fev.record(main)
             dev_ev[ds] = fev
@@ -459,35 +446,24 @@ class MVectorPredictor:
         zero padded to the longest item of the (global) batch; ``lens`` the true sample counts (None: every row is full
         length, i.e. no masking) or ``keep`` the precomputed device int32 mask lengths.  Returns the device tensor
         ``[B, embd_dim]`` (``out`` when given: a contiguous CUDA float32 ``[B, embd_dim]`` view to write into).  One fused
-        ``vp_embed_wave`` (front-end + backbone) per chunk of <= MAX_BATCH utterances; nothing is copied or synchronised."""
-        from . import _lib as L
+        front-end call over the whole batch, then one backbone program per chunk of <= MAX_BATCH utterances; nothing is
+        copied or synchronised."""
         assert wave_dev.is_cuda and wave_dev.dtype == torch.float32 and wave_dev.dim() == 2 and wave_dev.is_contiguous()
         B, Lp = wave_dev.shape
         assert lmax is None or lmax == Lp
         fz = self._audio_featurizer
         T = fz.num_frames(Lp)
-        desc = fz.feat_fun.desc
         if keep is None and lens is not None:
             keep = fz.keep_frames(torch.tensor([n / Lp for n in lens], dtype=torch.float32), T).to(wave_dev.device)
-        D, F = self.predictor.embd_dim, fz.feature_dim
+        D = self.predictor.embd_dim
         if out is not None:
             assert out.is_cuda and out.dtype == torch.float32 and tuple(out.shape) == (B, D) and out.is_contiguous()
         emb = out if out is not None else torch.empty(B, D, dtype=torch.float32, device=wave_dev.device)
         cb = self._chunk_size(B, T)
-        if desc.post == 1 and desc.top_db >= 0:         # MFCC: call-wide clamp -> front-end on the whole batch first
-            feats = fz.forward_keep(wave_dev, keep, group=group)
-            for lo in range(0, B, cb):
-                hi = min(lo + cb, B)
-                self.predictor.program(hi - lo, T).run(feats[lo:hi].contiguous(), emb[lo:hi])
-            return emb
-        eng = fz.engine
-        feats = torch.empty(cb * T * F, dtype=torch.float32, device=wave_dev.device)
-        scratch = torch.empty(max(int(L.lib().vp_frontend_scratch_floats(eng.handle, cb, Lp)), 1), dtype=torch.float32,
-                              device=wave_dev.device)
+        feats = fz.forward_keep(wave_dev, keep, group=group)
         for lo in range(0, B, cb):
             hi = min(lo + cb, B)
-            self.predictor.program(hi - lo, T).run_wave(wave_dev[lo:hi], None if keep is None else keep[lo:hi],
-                                                        feats[:(hi - lo) * T * F], scratch, emb[lo:hi])
+            self.predictor.program(hi - lo, T).run(feats[lo:hi], emb[lo:hi])
         return emb
 
     def predict(self, audio_data, sample_rate=16000):
