@@ -259,7 +259,9 @@ void vp_program_destroy(vp_program* p);
 /* feats [B,T,F] -> emb [B, embd_dim] */
 int vp_embed(vp_program* p, const float* feats, float* emb, void* stream);
 /* Same as vp_embed but brackets every op with CUDA events on `stream`, synchronises, and writes the per-op device
- * time in milliseconds to the HOST array ms_per_op[n_ops] (bench.py's live roofline measurement). */
+ * time in milliseconds to the HOST array ms_per_op[n_ops] (bench.py's live roofline measurement).  Ops that run as one
+ * launch -- a Res2Net chain of split-TF32 convs fused by vp_program_create -- book the launch's time on the chain's
+ * first op and about 0 on the others. */
 int vp_embed_profiled(vp_program* p, const float* feats, float* emb, void* stream, float* ms_per_op);
 /* op i of the program: kind, GEMM view (M rows, N = Cout, K = taps*Cin; K = 0 for non-conv ops), resolved engine */
 int vp_program_op_info(const vp_program* p, int32_t i, int32_t* kind, int64_t* M, int64_t* N, int64_t* K, int32_t* engine);
@@ -479,9 +481,10 @@ int vp_host_stage_h2d(const float* const* srcs, const int32_t* lens, int32_t n, 
 int vp_host_gather_streaming(int on);
 /* bytes of the handle's shared workspace arena right now */
 size_t vp_workspace_bytes(const vp_handle* h);
-/* number of kernel launches one vp_embed enqueues (bench.py's gpu_launches) */
+/* number of kernel launches one vp_embed enqueues (bench.py's gpu_launches): a fused Res2Net chain counts once */
 int32_t vp_program_launches(const vp_program* p);
-/* debugging / tests: copy a workspace region to a caller device buffer on the stream */
+/* debugging / tests: copy a region of the program's workspace, or of the amax slots behind it (uint32 slot q at byte
+ * offset round_up(workspace_bytes, 256) + 4 (q - 1)), to a caller device buffer on the stream */
 int vp_program_peek(vp_program* p, int64_t byte_offset, size_t nbytes, void* dst_device, void* stream);
 
 #ifdef __cplusplus

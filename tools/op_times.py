@@ -29,5 +29,9 @@ for o in acc:
     key = (o['kind'], o['engine'], o['M'], o['N'], o['K'])
     a = agg.setdefault(key, [0, 0.0]); a[0] += 1; a[1] += o['ms'] / 3
 tot = sum(v[1] for v in agg.values())
+# a fused Res2Net chain books its launch on the chain's first op and ~0 on the rest (vp_embed_profiled)
+chain = [o['ms'] for o in acc if o['kind'] == 1 and o['engine'] == 2 and o['N'] <= 64 and o['K'] == 3 * o['N']]
+if chain:
+    print('res2 chain convs (N <= 64, k3): %d ops, %.3f ms in all' % (len(chain), sum(chain) / 3))
 print('total %.3f ms' % tot, ' | '.join(f"{'tf32' if k[1] == 2 else 'fp16'} {k[2]}x{k[3]}x{k[4]}:{v[1]/v[0]:.3f}"
                                         for k, v in agg.items() if k[0] == 1 and k[1] in (2, 3)))

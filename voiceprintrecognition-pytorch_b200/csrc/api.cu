@@ -45,6 +45,9 @@ struct vp_program {
   vp_handle* h = nullptr;
   std::vector<vp_op> ops;
   std::vector<int> engines;   // resolved conv engine per op (VP_ENGINE_FFMA / VP_ENGINE_TC), 0 for non-conv
+  // fused Res2Net chains (res2_chain_len): chain[i] = n > 1 at the first op of a chain of n ops launched as one
+  // res2_chain_kernel, -1 at the chain's other ops, 0 elsewhere
+  std::vector<int> chain;
   size_t ws_bytes = 0, in_floats = 0, out_floats = 0;
   int launches = 0;
   int B = 0;                  // utterances (every op of a program agrees on it)
@@ -538,6 +541,48 @@ static int validate_op(vp_program* p, const vp_op& o, int i) {
   }
 }
 
+// A Res2Net chain op of the fused kernel: a tensor-core k3 reflect conv of width w = Cin = Cout (a multiple of 16, at most
+// 64) over frames, stride 1, pad = dilation, with the simple epilogue (bias, ReLU, post affine) and no fp16 scale input.
+static bool res2_op_ok(const vp_program* p, int i) {
+  const vp_op& o = p->ops[i];
+  if (o.kind != VP_OP_CONV || p->engines[i] != VP_ENGINE_TC) return false;
+  if (o.Fin != 1 || o.Fout != 1 || o.Tin != o.Tout || o.KT != 3 || o.KF != 1 || o.sT != 1 || o.sF != 1) return false;
+  if (o.pad_mode != VP_PAD_REFLECT || o.padT != o.dT || o.padF != 0) return false;
+  if (o.Cin != o.Cout || o.tc_bn != o.Cout || !res2_chain_supported(o.Cout, o.Tout, o.dT)) return false;
+  if (o.src2_mode == VP_SRC2_CONCAT || o.pre_s >= 0 || o.tc_kc != 0 || o.amax_in != 0) return false;
+  if (o.res != VP_BUF_NONE || o.gate != VP_BUF_NONE || o.ubias != VP_BUF_NONE || o.sum != VP_BUF_NONE) return false;
+  return (o.act == VP_ACT_NONE || o.act == VP_ACT_RELU) && o.act2 == VP_ACT_NONE;
+}
+
+// Length of the Res2Net chain starting at op i (0 when fewer than two ops): consecutive res2_op_ok ops of one geometry
+// and one activation (the kernel applies op 0's to every op),
+// op k reading column window k of one source tensor and writing window k of one destination tensor, every op after the
+// first adding the previous op's output (SRC2_ADD), one amax slot, and source and destination apart in memory.
+static int res2_chain_len(const vp_program* p, int i) {
+  const int n_ops = (int)p->ops.size();
+  if (!res2_op_ok(p, i) || p->ops[i].src2_mode != VP_SRC2_NONE) return 0;
+  const vp_op& f = p->ops[i];
+  const int w = f.Cout;
+  int n = 1;
+  while (n < RES2_MAX_OPS && i + n < n_ops && res2_op_ok(p, i + n)) {
+    const vp_op& o = p->ops[i + n];
+    const vp_op& q = p->ops[i + n - 1];
+    if (o.B != f.B || o.Tout != f.Tout || o.dT != f.dT || o.Cout != w || o.act != f.act || o.amax_out != f.amax_out) break;
+    if (o.src != f.src || o.in_ld != f.in_ld || o.in_coff != q.in_coff + w) break;
+    if (o.dst != f.dst || o.out_ld != f.out_ld || o.out_coff != q.out_coff + w) break;
+    if (o.src2_mode != VP_SRC2_ADD || o.src2 != q.dst || o.src2_ld != q.out_ld || o.src2_coff != q.out_coff) break;
+    ++n;
+  }
+  if (n < 2) return 0;
+  // the kernel reads op k + 1's source while it writes op k's output: the two views must not share a byte
+  const long long rows = (long long)f.B * f.Tout;
+  const int64_t s0 = f.src + 4 * (int64_t)f.in_coff, s1 = f.src + 4 * (int64_t)view_floats(rows, f.in_ld, f.in_coff + (n - 1) * w, w);
+  const int64_t d0 = f.dst + 4 * (int64_t)f.out_coff, d1 = f.dst + 4 * (int64_t)view_floats(rows, f.out_ld, f.out_coff + (n - 1) * w, w);
+  const bool src_ws = f.src >= 0, dst_ws = f.dst >= 0;
+  if (src_ws == dst_ws && (src_ws || f.src == f.dst) && s0 < d1 && d0 < s1) return 0;
+  return n;
+}
+
 int vp_program_create(vp_handle* h, const vp_op* ops, int32_t n_ops, size_t ws_bytes, size_t in_floats,
                       size_t out_floats, vp_program** out) {
   if (!h || !ops || n_ops < 1 || !out) return fail(h, VP_ERR_INVALID, "null/empty program");
@@ -591,6 +636,15 @@ int vp_program_create(vp_handle* h, const vp_op* ops, int32_t n_ops, size_t ws_b
     if (o.engine == VP_ENGINE_TC16 || (o.engine == VP_ENGINE_AUTO && ok16 && tc16_enabled())) p->engines[i] = VP_ENGINE_TC16;
     else if (o.engine == VP_ENGINE_TC || (o.engine == VP_ENGINE_AUTO && ok)) p->engines[i] = VP_ENGINE_TC;
     else p->engines[i] = VP_ENGINE_FFMA;
+  }
+  p->chain.assign(n_ops, 0);
+  for (int i = 0; i < n_ops;) {
+    const int n = res2_chain_len(p, i);
+    if (n < 2) { ++i; continue; }
+    p->chain[i] = n;
+    for (int k = 1; k < n; ++k) p->chain[i + k] = -1;
+    p->launches -= n - 1;
+    i += n;
   }
   if (cudaSetDevice(h->device) != cudaSuccess) { delete p; return fail(h, VP_ERR_CUDA, "cudaSetDevice"); }
   if (p->arena_need() > h->arena_bytes) {
@@ -663,6 +717,24 @@ static int run_ops(vp_program* p, const float* feats, float* emb, cudaStream_t s
   for (size_t i = 0; i < p->ops.size(); ++i) {
     const vp_op& o = p->ops[i];
     if (evs) CUDA_TRY(h, cudaEventRecord(evs[i], st));
+    if (p->chain[i] < 0) continue;               // launched with its chain's first op
+    if (p->chain[i] > 0) {
+      Res2Args a{};
+      a.n_ops = p->chain[i];
+      for (int k = 0; k < a.n_ops; ++k) {
+        ConvParams c;
+        fill_conv(p, p->ops[i + k], feats, emb, c);
+        a.src[k] = c.src + c.in_coff; a.dst[k] = c.dst + c.out_coff; a.w_tc[k] = c.w_tc;
+        a.bias[k] = c.bias; a.post_s[k] = c.post_s; a.post_h[k] = c.post_h;
+        if (k == 0) {
+          a.amax_out = c.amax_out;
+          a.W = c.N; a.B = c.B; a.T = c.Tout; a.d = c.dT; a.in_ld = c.in_ld; a.out_ld = c.out_ld;
+          a.relu = c.act == VP_ACT_RELU;
+        }
+      }
+      CUDA_TRY(h, launch_res2_chain(a, st));
+      continue;
+    }
     switch (o.kind) {
       case VP_OP_CONV:
       case VP_OP_CONV_C1: {
@@ -993,7 +1065,7 @@ int vp_pcm_decode(vp_handle* h, const uint8_t* data, int64_t nbytes, const vp_pc
 
 int vp_program_peek(vp_program* p, int64_t off, size_t nbytes, void* dst, void* stream) {
   if (!p || !dst) return VP_ERR_INVALID;
-  if (off < 0 || (size_t)off + nbytes > p->ws_bytes) return fail(p->h, VP_ERR_INVALID, "peek out of range");
+  if (off < 0 || (size_t)off + nbytes > p->arena_need()) return fail(p->h, VP_ERR_INVALID, "peek out of range");
   CUDA_TRY(p->h, cudaMemcpyAsync(dst, p->h->d_arena + off, nbytes, cudaMemcpyDeviceToDevice, (cudaStream_t)stream));
   return VP_OK;
 }

@@ -101,8 +101,7 @@ __device__ __forceinline__ float tf32_rna(float x) {
 // D[64 x BN] (+)= A[64 x 8|16] * B[BN x 8|16]^T for one warpgroup.  BN is a multiple of 16 up to 128: it is issued as
 // n128, or as n64 / n32 / n16 pieces (B rows of a piece start at a multiple of 16 rows = 2 KB: swizzle atoms stay aligned).
 template <int BN, bool F16>
-__device__ __forceinline__ void mma_tile(float* d, uint32_t a, uint32_t b, uint32_t scale_d) {
-  const uint64_t da = smem_desc(a);
+__device__ __forceinline__ void mma_tile_desc(float* d, uint64_t da, uint32_t b, uint32_t scale_d) {
   if constexpr (BN == 128) {
     if constexpr (F16) wgmma_f16_n128(d, da, smem_desc(b), scale_d);
     else wgmma_tf32_n128(d, da, smem_desc(b), scale_d);
@@ -121,6 +120,10 @@ __device__ __forceinline__ void mma_tile(float* d, uint32_t a, uint32_t b, uint3
       else wgmma_tf32_n16(d + o16 / 2, da, smem_desc(b + o16 * 128), scale_d);
     }
   }
+}
+template <int BN, bool F16>
+__device__ __forceinline__ void mma_tile(float* d, uint32_t a, uint32_t b, uint32_t scale_d) {
+  mma_tile_desc<BN, F16>(d, smem_desc(a), b, scale_d);
 }
 
 __device__ __noinline__ float2 act2_slow(float2 v, int act) {
@@ -148,6 +151,16 @@ __device__ __forceinline__ Epi make_epi(const ConvParams& p, float descale) {
   e.need_urow = (p.gate != nullptr) || (p.ubias != nullptr);
   e.descale = descale;
   return e;
+}
+
+// The head of the simple epilogue, shared by store_tile's fast path and the fused Res2Net chain so that the two cannot
+// drift: acc * descale + bias in one rounding, optional clamp to [0, hi], optional BN affine.
+__device__ __forceinline__ float2 epi_head(float2 x, float descale, float2 b2, bool relu, float hi, bool post, float2 s2,
+                                           float2 h2) {
+  x.x = fmaf(x.x, descale, b2.x); x.y = fmaf(x.y, descale, b2.y);      // descale == 1 on the tf32 path
+  if (relu) { x.x = fminf(fmaxf(x.x, 0.f), hi); x.y = fminf(fmaxf(x.y, 0.f), hi); }
+  if (post) { x.x = fmaf(x.x, s2.x, h2.x); x.y = fmaf(x.y, s2.y, h2.y); }
+  return x;
 }
 
 // Residual tiles are pure streaming: pull tile gg's residual rows (this consumer warp's 16) into the L2 while the
@@ -191,10 +204,8 @@ __device__ __forceinline__ void store_tile(const ConvParams& p, const Epi& e, co
       }
 #pragma unroll
       for (int h = 0; h < 2; ++h) {
-        float2 x = make_float2(res[4 * j + 2 * h], res[4 * j + 2 * h + 1]);
-        x.x = fmaf(x.x, descale, b2.x); x.y = fmaf(x.y, descale, b2.y);      // descale == 1 on the tf32 path
-        if (e.relu) { x.x = fminf(fmaxf(x.x, 0.f), e.hi1); x.y = fminf(fmaxf(x.y, 0.f), e.hi1); }
-        if (p.post_s) { x.x = fmaf(x.x, s2.x, h2.x); x.y = fmaf(x.y, s2.y, h2.y); }
+        float2 x = epi_head(make_float2(res[4 * j + 2 * h], res[4 * j + 2 * h + 1]), descale, b2, e.relu, e.hi1,
+                            p.post_s != nullptr, s2, h2);
         if (rp) { x.x += rr[h].x; x.y += rr[h].y; }
         if (e.relu2) { x.x = fminf(fmaxf(x.x, 0.f), e.hi2); x.y = fminf(fmaxf(x.y, 0.f), e.hi2); }
         *reinterpret_cast<float2*>(o + 8 * j + h * o8) = x;
@@ -752,6 +763,225 @@ __global__ void __launch_bounds__(W_THREADS, 1) conv_tc16_wide_kernel(const __gr
   if (p.amax_out) amax_commit(p.amax_out, tmax);     // one atomicMax per consumer warp per launch
 }
 
+// ---------------------------------------------------------------------------------------------------------------------
+// Fused Res2Net chain (launch_res2_chain; api.cu res2_chain_len picks the ops): y_j = conv_j(t1_j + y_{j-1}), n_ops
+// dependent k3 reflect-padded convs of width W <= 64 at dilation d, one utterance per CTA (persistent over B).
+// The per-op path spends 21 launches per ECAPA forward on them, each 596 128 x 64 tiles with 6 K blocks; here y_{j-1}
+// never leaves the SM and each t1 slice is read once.
+//
+// x_j = t1_j + y_{j-1} lives in shared memory, already split: an fp32 hi plane (tf32_rna(x)) and a lo plane (x - hi),
+// each [W / 4 column chunks][rows][4 floats] -- the no-swizzle K-major core-matrix layout, whose descriptor may start at
+// any row, so the A operand of tap kt for output rows t.. is the plane at row t + kt d.  Plane row t + d holds frame t;
+// the d rows on either side hold the reflected frames, written alongside their sources.  The last row block reads up to
+// 63 rows past a chunk's end: those rows feed only output rows >= T, which are never stored nor folded into the amax.
+//   warps 0-11 consumers : three warpgroups, warpgroup g owning 64-row blocks g and g + 3 (T <= 384), issue the same
+//                          wgmma sequence as conv_tc_kernel<*, false, W> per output row (tap-major K blocks of 32,
+//                          lo*hi, hi*lo, hi*hi per k8 into one accumulator, zero A past K), then, after all warpgroups
+//                          are done reading the planes, run the epilogue (epi_head), store y_j and overwrite the planes
+//                          with x_{j+1} = t1_{j+1} + y_j in place
+//   warp 12 thread 0     : streams op j's split-TF32 weight image (w_tc, BN = W) one K block per stage, cp.async.bulk
+constexpr int R2_WG = 3;
+constexpr int R2_RB = 2;
+constexpr int R2_CONSUMERS = R2_WG * 128;
+constexpr int R2_THREADS = R2_CONSUMERS + 32;
+constexpr int R2_MAX_T = R2_WG * R2_RB * 64;
+constexpr int R2_MAX_STAGES = 4;
+constexpr int R2_ZERO = 2048;            // zero A operand of the k8 steps past K: 64 rows x 2 chunks, LBO 1 KB
+
+// K-major, no-swizzle descriptor: core matrices of 8 rows x 16 B, SBO = 128 B between 8-row groups, LBO between the
+// two 16-byte K chunks of a k8 step
+__device__ __forceinline__ uint64_t plane_desc(uint32_t addr, uint32_t lbo) {
+  return (uint64_t)((addr >> 4) & 0x3FFF) | ((uint64_t)((lbo >> 4) & 0x3FFF) << 16) | (8ull << 32);
+}
+__device__ __forceinline__ void consumers_sync() { asm volatile("bar.sync 1, %0;" ::"n"(R2_CONSUMERS) : "memory"); }
+
+template <int W>
+__global__ void __launch_bounds__(R2_THREADS, 1) res2_chain_kernel(const __grid_constant__ Res2Args a) {
+  static_assert(W % 16 == 0 && W >= 16 && W <= 64, "chain width");
+  constexpr int KB = (3 * W + BK - 1) / BK;                    // K blocks per conv
+  constexpr uint32_t b_tile = (uint32_t)W * 128u, stage_bytes = 2u * b_tile;
+  pdl_launch_dependents();
+  extern __shared__ uint8_t smem_raw[];
+  __shared__ __align__(8) uint64_t bars[2 * R2_MAX_STAGES];
+  const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
+  const int S = a.stages, T = a.T, d = a.d;
+  const uint32_t base = (smem_u32(smem_raw) + 1023u) & ~1023u;
+  const uint32_t zero = base + S * stage_bytes;
+  const uint32_t lbo = (uint32_t)a.rows * 16u;
+  const uint32_t hi_pl = zero + R2_ZERO, lo_pl = hi_pl + (W / 4) * lbo;
+  const uint32_t full0 = smem_u32(&bars[0]), empty0 = smem_u32(&bars[R2_MAX_STAGES]);
+  if (threadIdx.x == 0) {
+    for (int s = 0; s < S; ++s) {
+      mbar_init(full0 + 8 * s, 1);
+      mbar_init(empty0 + 8 * s, R2_CONSUMERS / 32);
+    }
+    asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory");
+  }
+  for (int i = threadIdx.x; i < R2_ZERO / 16; i += R2_THREADS)
+    asm volatile("st.shared.v4.u32 [%0], {%1, %1, %1, %1};" ::"r"(zero + 16 * i), "r"(0u) : "memory");
+  fence_proxy_async();
+  __syncthreads();
+  // before the first global read of any thread, the weight producer's included: the weight image is written by
+  // vp_weights_load's synchronous copy today, but a device-side writer of the blob would be ordered by this wait
+  pdl_wait();
+
+  if (warp == R2_CONSUMERS / 32) {
+    // =========================== weight producer ===========================
+    if (lane != 0) return;
+    int s = 0;
+    uint32_t ph = 0;
+    for (int b = blockIdx.x; b < a.B; b += gridDim.x)
+      for (int j = 0; j < a.n_ops; ++j)
+        for (int kb = 0; kb < KB; ++kb) {
+          mbar_wait(empty0 + 8 * s, ph ^ 1);
+          mbar_expect_tx(full0 + 8 * s, stage_bytes);
+          bulk_copy_g2s(base + s * stage_bytes, reinterpret_cast<const uint8_t*>(a.w_tc[j]) + (size_t)kb * stage_bytes,
+                        stage_bytes, full0 + 8 * s);
+          if (++s == S) { s = 0; ph ^= 1u; }
+        }
+    return;
+  }
+
+  // =========================== consumers ===========================
+  const int wg = warp >> 2, q4 = lane & 3;
+  const int rw = 16 * (warp & 3) + (lane >> 2);                 // fragment rows rw and rw + 8 of a 64-row block
+  const int nrb = (T + 63) >> 6;
+  // row blocks of this warpgroup, as a warp-uniform value: a branch around the wgmmas that the compiler must treat as
+  // divergent makes it serialise them
+  const int mine = __shfl_sync(0xffffffffu, nrb > wg + R2_WG ? 2 : (nrb > wg ? 1 : 0), 0);
+  // writes the split of x (frame t, columns n, n + 1) into both planes, and into the rows that reflect frame t
+  auto put2 = [&](int t, int n, float2 x) {
+    const float2 h = make_float2(tf32_rna(x.x), tf32_rna(x.y));
+    const float2 l = make_float2(x.x - h.x, x.y - h.y);
+    const uint32_t col = (uint32_t)(n >> 2) * lbo + (uint32_t)(n & 3) * 4u;
+    int rows[3] = {t + d, (t >= 1 && t <= d) ? d - t : -1, (t >= T - 1 - d && t <= T - 2) ? 2 * (T - 1) - t + d : -1};
+#pragma unroll
+    for (int i = 0; i < 3; ++i) {
+      if (rows[i] < 0) continue;
+      const uint32_t o = col + (uint32_t)rows[i] * 16u;
+      // no "memory" clobber: global loads may be hoisted above these stores; fence_proxy_async + consumers_sync order
+      // them before the wgmmas that read the planes
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(hi_pl + o), "f"(h.x), "f"(h.y));
+      asm volatile("st.shared.v2.f32 [%0], {%1, %2};" ::"r"(lo_pl + o), "f"(l.x), "f"(l.y));
+    }
+  };
+  float tmax = 0.f;
+  int s = 0;
+  uint32_t sph = 0;
+  for (int b = blockIdx.x; b < a.B; b += gridDim.x) {
+    const size_t row0 = (size_t)b * T;
+    // x_0 = op 0's source: a warp covers 8 frames x 4 chunks (conflict-free plane stores, 64 B global row segments)
+    const int n_x0 = ((T + 7) >> 3) * 8 * (W / 4);
+    for (int i0 = threadIdx.x; i0 < n_x0; i0 += 4 * R2_CONSUMERS) {
+      float4 v[4];
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {                              // four loads in flight before the first store
+        const int i = i0 + u * R2_CONSUMERS, t = (i & 7) + 8 * (i / (8 * (W / 4))), c = (i >> 3) % (W / 4);
+        v[u] = make_float4(0.f, 0.f, 0.f, 0.f);
+        if (i < n_x0 && t < T) v[u] = __ldg(reinterpret_cast<const float4*>(a.src[0] + (row0 + t) * a.in_ld + 4 * c));
+      }
+#pragma unroll
+      for (int u = 0; u < 4; ++u) {
+        const int i = i0 + u * R2_CONSUMERS, t = (i & 7) + 8 * (i / (8 * (W / 4))), c = (i >> 3) % (W / 4);
+        if (i >= n_x0 || t >= T) continue;
+        put2(t, 4 * c, make_float2(v[u].x, v[u].y));
+        put2(t, 4 * c + 2, make_float2(v[u].z, v[u].w));
+      }
+    }
+    fence_proxy_async();
+    consumers_sync();
+    for (int j = 0; j < a.n_ops; ++j) {
+      const bool last = j + 1 == a.n_ops;
+      if (!last)                                                 // the epilogue's t1_{j+1} reads become L2 hits
+        for (int t = threadIdx.x; t < T; t += R2_CONSUMERS)
+          for (int c = 0; c < W; c += 32)
+            asm volatile("prefetch.global.L2 [%0];" ::"l"(a.src[j + 1] + (row0 + t) * a.in_ld + c));
+      float acc[R2_RB][W / 2];
+      int prev = -1;
+      for (int kb = 0; kb < KB; ++kb) {
+        mbar_wait(full0 + 8 * s, sph);
+        const uint32_t b_hi = base + s * stage_bytes, b_lo = b_hi + b_tile;
+        wgmma_fence();
+#pragma unroll
+        for (int r = 0; r < R2_RB; ++r) {
+          const int rb = wg + R2_WG * r;
+          if (r >= mine) continue;
+#pragma unroll
+          for (int kk = 0; kk < 4; ++kk) {
+            const int k = kb * BK + kk * 8;
+            uint64_t dh = plane_desc(zero, 1024u), dl = dh;
+            if (k < 3 * W) {
+              const int kt = k / W, ci = k - kt * W;
+              const uint32_t o = (uint32_t)(ci >> 2) * lbo + (uint32_t)(64 * rb + kt * d) * 16u;
+              dh = plane_desc(hi_pl + o, lbo);
+              dl = plane_desc(lo_pl + o, lbo);
+            }
+            mma_tile_desc<W, false>(acc[r], dl, b_hi + kk * 32, (kb != 0) || (kk != 0));
+            mma_tile_desc<W, false>(acc[r], dh, b_lo + kk * 32, 1);
+            mma_tile_desc<W, false>(acc[r], dh, b_hi + kk * 32, 1);
+          }
+        }
+        wgmma_commit();
+        if (prev >= 0) {
+          wgmma_wait<1>();
+          if (lane == 0) mbar_arrive(empty0 + 8 * prev);
+        }
+        prev = s;
+        if (++s == S) { s = 0; sph ^= 1u; }
+      }
+      wgmma_wait<0>();
+#pragma unroll
+      for (int r = 0; r < R2_RB; ++r) fence_regs(acc[r]);
+      if (lane == 0) mbar_arrive(empty0 + 8 * prev);
+      consumers_sync();                                          // every warpgroup is done reading x_j
+      const float* bias = a.bias[j];
+      const float* ps = a.post_s[j];
+      const float* ph = a.post_h[j];
+      float* dst = a.dst[j];
+      const float* nxt = last ? nullptr : a.src[j + 1];
+#pragma unroll
+      for (int r = 0; r < R2_RB; ++r) {
+        const int rb = wg + R2_WG * r;
+        if (rb >= nrb) continue;
+        float2 t1n[2][W / 8];                                   // t1_{j+1} of both fragment rows, loaded up front
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int t = 64 * rb + rw + 8 * h;
+#pragma unroll
+          for (int jj = 0; jj < W / 8; ++jj)
+            t1n[h][jj] = (last || t >= T) ? make_float2(0.f, 0.f)
+                                          : __ldg(reinterpret_cast<const float2*>(nxt + (row0 + t) * a.in_ld + 8 * jj + 2 * q4));
+        }
+#pragma unroll
+        for (int h = 0; h < 2; ++h) {
+          const int t = 64 * rb + rw + 8 * h;
+          if (t >= T) continue;
+          float* o = dst + (row0 + t) * a.out_ld;
+#pragma unroll
+          for (int jj = 0; jj < W / 8; ++jj) {
+            const int n = 8 * jj + 2 * q4;
+            float2 b2 = make_float2(0.f, 0.f), s2 = make_float2(1.f, 1.f), h2 = b2;
+            if (bias) b2 = __ldg(reinterpret_cast<const float2*>(bias + n));
+            if (ps) {
+              s2 = __ldg(reinterpret_cast<const float2*>(ps + n));
+              h2 = __ldg(reinterpret_cast<const float2*>(ph + n));
+            }
+            const float2 y = epi_head(make_float2(acc[r][4 * jj + 2 * h], acc[r][4 * jj + 2 * h + 1]), 1.f, b2, a.relu,
+                                      INFINITY, ps != nullptr, s2, h2);
+            *reinterpret_cast<float2*>(o + n) = y;
+            tmax = fmaxf(tmax, fmaxf(fabsf(y.x), fabsf(y.y)));
+            if (!last)                                           // t1_{j+1} + y_j, as conv_tc_kernel<1>'s gather adds
+              put2(t, n, make_float2(t1n[h][jj].x + y.x, t1n[h][jj].y + y.y));
+          }
+        }
+      }
+      fence_proxy_async();                                       // plane stores -> visible to the tensor core
+      consumers_sync();
+    }
+  }
+  if (a.amax_out) amax_commit(a.amax_out, tmax);
+}
+
 }  // namespace tc
 
 // Host-visible tiling rule (mirrored by the Python packer mvector/engine.py::tc_tile_n).  The accumulator lives in the
@@ -914,6 +1144,60 @@ static cudaError_t launch_conv_tc16_wide(const ConvParams& p, const float* w_tc1
 cudaError_t launch_conv_tc16(const ConvParams& p, const float* w_tc16, float descale, cudaStream_t stream) {
   if (tc16_wide_ok(p)) return launch_conv_tc16_wide(p, w_tc16, descale, stream);
   return launch_conv_tc_impl(p, w_tc16, true, descale, stream);
+}
+
+// Fused Res2Net chain: plane rows (T + 2d, rounded to 4 mod 8 so that a quad's two 16-byte chunks of one row fall in
+// different bank halves) and the dynamic shared memory of `stages` weight stages.  The planes are what bounds T: at
+// W = 64 two stages leave room for T + 2d <= 380, i.e. T <= 372 at ECAPA's largest dilation (3.7 s at a 10 ms hop).
+// Longer utterances run the per-op path.
+static int res2_rows(int T, int d) { return (T + 2 * d + 3) / 8 * 8 + 4; }
+static size_t res2_smem(int W, int T, int d, int stages) {
+  return 1024 + (size_t)stages * 2 * W * 128 + tc::R2_ZERO + 2 * (size_t)(W / 4) * res2_rows(T, d) * 16 + 1024;
+}
+static constexpr size_t R2_SMEM_MAX = 226 * 1024;   // + the static barriers, within the 227 KB opt-in limit
+
+bool res2_chain_supported(int W, int T, int d) {
+  if (W % 16 != 0 || W < 16 || W > 64 || T > tc::R2_MAX_T || d < 1 || d >= T) return false;
+  return res2_smem(W, T, d, 2) <= R2_SMEM_MAX;
+}
+
+template <int W>
+static cudaError_t launch_res2_w(const cudaLaunchConfig_t& cfg, const Res2Args& a) {
+  static PerDeviceSmem once;
+  if (once.need(cfg.dynamicSmemBytes)) {
+    cudaError_t e = cudaFuncSetAttribute(tc::res2_chain_kernel<W>, cudaFuncAttributeMaxDynamicSharedMemorySize,
+                                         (int)cfg.dynamicSmemBytes);
+    if (e != cudaSuccess) return e;
+    once.set(cfg.dynamicSmemBytes);
+  }
+  return cudaLaunchKernelEx(&cfg, tc::res2_chain_kernel<W>, a);
+}
+
+cudaError_t launch_res2_chain(Res2Args a, cudaStream_t stream) {
+  if (!res2_chain_supported(a.W, a.T, a.d) || a.n_ops < 1 || a.n_ops > RES2_MAX_OPS) return cudaErrorInvalidConfiguration;
+  a.rows = res2_rows(a.T, a.d);
+  a.stages = 2;
+  while (a.stages < tc::R2_MAX_STAGES && res2_smem(a.W, a.T, a.d, a.stages + 1) <= R2_SMEM_MAX) ++a.stages;
+  const int sms = sm_count();
+  cudaLaunchConfig_t cfg{};
+  cfg.gridDim = dim3(sms < a.B ? sms : a.B);
+  cfg.blockDim = dim3(tc::R2_THREADS);
+  cfg.dynamicSmemBytes = res2_smem(a.W, a.T, a.d, a.stages);
+  cfg.stream = stream;
+  cudaLaunchAttribute attr[1];
+  attr[0].id = cudaLaunchAttributeProgrammaticStreamSerialization;
+  attr[0].val.programmaticStreamSerializationAllowed = pdl_enabled();
+  cfg.attrs = attr;
+  cfg.numAttrs = 1;
+  cudaError_t e;
+  switch (a.W) {
+    case 16: e = launch_res2_w<16>(cfg, a); break;
+    case 32: e = launch_res2_w<32>(cfg, a); break;
+    case 48: e = launch_res2_w<48>(cfg, a); break;
+    default: e = launch_res2_w<64>(cfg, a); break;
+  }
+  if (e != cudaSuccess) return e;
+  return cudaGetLastError();
 }
 
 }  // namespace vpb

@@ -137,5 +137,17 @@ cudaError_t launch_conv_tc(const ConvParams& p, cudaStream_t stream);
 // two-term FP16 split of the same engine (VP_ENGINE_TC16)
 bool conv_tc16_supported(const ConvParams& p);
 cudaError_t launch_conv_tc16(const ConvParams& p, const float* w_tc16, float descale, cudaStream_t stream);
+// fused Res2Net chain of the same engine (res2_chain_kernel): n_ops dependent k3 reflect convs of width W on one
+// utterance per CTA, op j reading src[j] (+ op j-1's output) and writing dst[j]; pointers include the column offsets
+constexpr int RES2_MAX_OPS = 15;
+struct Res2Args {
+  const float* src[RES2_MAX_OPS]; float* dst[RES2_MAX_OPS]; const float* w_tc[RES2_MAX_OPS];
+  const float* bias[RES2_MAX_OPS]; const float* post_s[RES2_MAX_OPS]; const float* post_h[RES2_MAX_OPS];
+  unsigned* amax_out;
+  int n_ops, W, B, T, d, in_ld, out_ld, relu;
+  int rows, stages;    // set by the launcher: plane rows, weight stages
+};
+bool res2_chain_supported(int W, int T, int d);
+cudaError_t launch_res2_chain(Res2Args a, cudaStream_t stream);
 
 }  // namespace vpb
