@@ -157,6 +157,49 @@ int vp_mfcc_finish(vp_handle* h, int32_t B, int32_t Lpad, const int32_t* keep_fr
 int vp_frontend_plan_info(const vp_handle* h, int32_t B, int32_t Lpad, int32_t stage, int32_t* info);
 
 /* ------------------------------------------------------------------------------------------------------------
+ * Hugging Face wav2vec 2.0 / WavLM front-end (use_hf_model, featurizer.py:25-38,65-73).  The reference keeps only
+ * `extract_features` of the model, which is the processor's normalisation followed by the convolutional feature encoder
+ * and the feature projection's LayerNorm:
+ *   x = do_normalize ? (w - mean(w)) / sqrt(var(w) + 1e-7) : w            numpy float32, per row (Wav2Vec2FeatureExtractor)
+ *   h = conv_l(h), no padding, bias iff conv_bias, then
+ *         norm 0 ("group"): layer 0 -> GroupNorm(one group per channel, over time, norm_eps) -> GELU; others -> GELU
+ *         norm 1 ("layer"): every layer -> LayerNorm over channels (norm_eps) -> GELU
+ *   f = LayerNorm(conv_dim[n - 1], proj_eps)(h)
+ * then the CMN and keep mask of every front-end.  vp_frontend_set_hf makes this the configured front-end (replacing
+ * any other, and vp_frontend_set replaces it): vp_features, vp_features_each, vp_frontend_scratch_floats,
+ * vp_num_frames, vp_feature_dim and vp_frontend_plan_info then serve it; vp_mfcc_mel / vp_mfcc_finish and
+ * vp_frontend_set_options refuse it.  The handle owns the encoder's weights (front-end state, not the backbone arena).
+ *   frames: T_0 = n < k_0 ? 0 : (n - k_0) / s_0 + 1, T_l = T_{l-1} < k_l ? 0 : (T_{l-1} - k_l) / s_l + 1; a call needs
+ *           T_{n-1} >= 1 (400 samples for the base geometry) and fails with VP_ERR_INVALID before any launch otherwise.
+ *   layer 0 needs k_0 a multiple of s_0 (it runs as a k_0 / s_0-tap conv over rows of s_0 samples, s_0 <= 16); every
+ *   layer's channels are multiples of 4 in [16, 1024].  The convolutions run on the split-TF32 tensor-core engine.
+ *   Rows are independent: a row's features depend on its own samples and (padded call) the padded length only, never
+ *   on the other rows or on the slicing below.  The call runs over slices of rows so that its scratch stays below
+ *   VP_HF_SCRATCH_CAP floats (1 GiB) whatever B is (one row per slice when a single row needs more: about 80 s of
+ *   16 kHz audio at 512 channels); vp_frontend_scratch_floats gives the exact need.
+ * ---------------------------------------------------------------------------------------------------------- */
+#define VP_HF_MAX_LAYERS 8
+#define VP_HF_SCRATCH_CAP ((size_t)1 << 28)
+enum { VP_HF_NORM_GROUP = 0, VP_HF_NORM_LAYER = 1 };
+typedef struct vp_hf_desc {
+  int32_t n_layers;                        /* conv layers, 1 .. VP_HF_MAX_LAYERS */
+  int32_t conv_dim[VP_HF_MAX_LAYERS];      /* output channels of each layer */
+  int32_t conv_kernel[VP_HF_MAX_LAYERS];
+  int32_t conv_stride[VP_HF_MAX_LAYERS];
+  int32_t conv_bias;                       /* 1: every conv has a bias */
+  int32_t norm;                            /* VP_HF_NORM_* (feat_extract_norm) */
+  int32_t do_normalize;                    /* 1: the processor's zero-mean unit-variance row normalisation */
+  float   norm_eps;                        /* the conv layers' GroupNorm / LayerNorm eps (1e-5) */
+  float   proj_eps;                        /* feature_projection.layer_norm eps (config.layer_norm_eps) */
+} vp_hf_desc;
+int32_t vp_sizeof_hf_desc(void);        /* binding self-check: sizeof(vp_hf_desc) */
+/* Host pointers, copied: conv_w[l] is layer l's weight [conv_dim[l], C_in, conv_kernel[l]] (C_in = 1 for layer 0,
+ * conv_dim[l-1] after), conv_b[l] its bias [conv_dim[l]] (NULL entries when !conv_bias); norm_w / norm_b[l] the affine
+ * of layer l's norm (only [0] for norm 0); proj_w / proj_b the projection LayerNorm's [conv_dim[n - 1]]. */
+int vp_frontend_set_hf(vp_handle* h, const vp_hf_desc* desc, const float* const* conv_w, const float* const* conv_b,
+                       const float* const* norm_w, const float* const* norm_b, const float* proj_w, const float* proj_b);
+
+/* ------------------------------------------------------------------------------------------------------------
  * Backbone (seam 2).  The host (Python mirror of the reference's mvector/models modules) lowers a model + a concrete (B, T) to a
  * straight-line program of fused ops over a workspace arena; weights live in one packed arena uploaded once.
  * Activations are channel-last: 1-D maps are [B, T, C], 2-D maps are [B, T, F, C] (T = time = conv2d W axis,
@@ -171,7 +214,8 @@ enum {                       /* vp_op.kind */
   VP_OP_POOL2D = 6           /* KTxKF max / average pooling on a channel-last 2-D map (res2net.py:33-34,105); mode 0 = max
                                 (implicit -inf padding), 1 = average with count_include_pad (zero padding, divide by KT*KF) */
 };
-enum { VP_ACT_NONE = 0, VP_ACT_RELU = 1, VP_ACT_HARDTANH20 = 2, VP_ACT_SIGMOID = 3, VP_ACT_TANH = 4, VP_ACT_SILU = 5 };
+enum { VP_ACT_NONE = 0, VP_ACT_RELU = 1, VP_ACT_HARDTANH20 = 2, VP_ACT_SIGMOID = 3, VP_ACT_TANH = 4, VP_ACT_SILU = 5,
+       VP_ACT_GELU = 6 };          /* GELU: exact erf form 0.5 v (1 + erf(v / sqrt 2)), torch's approximate='none' */
 enum { VP_PAD_ZERO = 0, VP_PAD_REFLECT = 1 };
 enum { VP_SRC2_NONE = 0, VP_SRC2_ADD = 1, VP_SRC2_CONCAT = 2 };
 enum {                       /* VP_OP_COLSTATS modes (op.mode) */

@@ -1,5 +1,5 @@
-"""Tiny workload for compute-sanitizer (memcheck / racecheck): small-config ECAPA + CAM++ from waveforms, and a small
-fused Res2Net chain."""
+"""Tiny workload for compute-sanitizer (memcheck / racecheck): small-config ECAPA + CAM++ from waveforms, a small
+fused Res2Net chain and a small HF wav2vec 2.0 / WavLM front-end."""
 import sys
 sys.path.insert(0, '.'); sys.path.insert(0, 'tests')
 import json, numpy as np, torch
@@ -28,4 +28,16 @@ import test_gpu_res2_chain as r2
 for tracked in (False, True):
     fused, ref, launches, _, slot = r2._run(8, 130, 32, 2, 3, tracked=tracked)
     print('res2 chain', 'tracked' if tracked else 'untracked', launches, slot, flush=True)
+# a small HF wav2vec 2.0 front-end (hf.cu), padded and ragged, both norms
+import tempfile
+from hf_writer import write_hf_dir
+for norm in ('group', 'layer'):
+    with tempfile.TemporaryDirectory() as td:
+        write_hf_dir(td, model_type='wav2vec2' if norm == 'group' else 'wavlm', norm=norm, conv_dim=(32,) * 7,
+                     conv_bias=norm == 'layer', seed=1)
+        fz = AudioFeaturizer(td, use_hf_model=True)
+        w = torch.randn(3, 4001, device='cuda') * 0.1
+        f = fz(w, torch.tensor([1.0, 0.5, 0.8]))
+        fe, tb = fz.forward_each(w, [4001, 400, 2999])
+        print('hf', norm, tuple(f.shape), tuple(fe.shape), tb.tolist(), flush=True)
 print('done')

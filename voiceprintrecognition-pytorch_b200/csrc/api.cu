@@ -39,6 +39,7 @@ struct vp_handle {
   double* d_mel_w = nullptr;   // the bank's weights widened to fp64, as the mel accumulation consumes them
   int mel_nw = 0;
   float* d_dct = nullptr;
+  HfState* hf = nullptr;       // the HF wav2vec 2.0 / WavLM front-end (vp_frontend_set_hf) instead of the above
 };
 
 struct vp_program {
@@ -97,6 +98,7 @@ int vp_abi_version(void) { return VP_ABI_VERSION; }
 int32_t vp_sizeof_op(void) { return (int32_t)sizeof(vp_op); }
 int32_t vp_sizeof_frontend_desc(void) { return (int32_t)sizeof(vp_frontend_desc); }
 int32_t vp_sizeof_frontend_options(void) { return (int32_t)sizeof(vp_frontend_options); }
+int32_t vp_sizeof_hf_desc(void) { return (int32_t)sizeof(vp_hf_desc); }
 
 int vp_create(int device, vp_handle** out) {
   if (!out) return VP_ERR_INVALID;
@@ -121,6 +123,8 @@ static void free_frontend(vp_handle* h) {
   h->d_dct = nullptr;
   h->d_window = nullptr; h->d_twiddle = nullptr; h->d_mel_start = h->d_mel_count = h->d_mel_off = nullptr;
   h->d_mel_w = nullptr;
+  hf_destroy(h->hf);
+  h->hf = nullptr;
   h->fe_set = false;
 }
 
@@ -196,9 +200,32 @@ int vp_frontend_set(vp_handle* h, const vp_frontend_desc* d, const float* window
   return VP_OK;
 }
 
+int vp_frontend_set_hf(vp_handle* h, const vp_hf_desc* d, const float* const* conv_w, const float* const* conv_b,
+                       const float* const* norm_w, const float* const* norm_b, const float* proj_w, const float* proj_b) {
+  if (!h || !d || !conv_w || !proj_w || !proj_b) return fail(h, VP_ERR_INVALID, "null argument");
+  const char* derr = hf_desc_error(*d);
+  if (*derr) return fail(h, VP_ERR_UNSUPPORTED, "HF front-end: %s", derr);
+  for (int l = 0; l < d->n_layers; ++l) {
+    if (!conv_w[l] || (d->conv_bias && (!conv_b || !conv_b[l])))
+      return fail(h, VP_ERR_INVALID, "HF front-end: layer %d conv weight / bias missing", l);
+    if ((d->norm == VP_HF_NORM_LAYER || l == 0) && (!norm_w || !norm_b || !norm_w[l] || !norm_b[l]))
+      return fail(h, VP_ERR_INVALID, "HF front-end: layer %d norm affine missing", l);
+  }
+  CUDA_TRY(h, cudaSetDevice(h->device));
+  free_frontend(h);
+  HfState* s = nullptr;
+  CUDA_TRY(h, hf_create(*d, conv_w, conv_b, norm_w, norm_b, proj_w, proj_b, &s));
+  h->hf = s;
+  h->fe = vp_frontend_desc{};
+  h->fe_opt = vp_frontend_options{VP_FRAME_DEFAULT, 0, 1.0};
+  h->fe_set = true;
+  return VP_OK;
+}
+
 int vp_frontend_set_options(vp_handle* h, const vp_frontend_options* o) {
   if (!h || !o) return fail(h, VP_ERR_INVALID, "null argument");
   if (!h->fe_set) return fail(h, VP_ERR_INVALID, "front-end not configured (vp_frontend_set)");
+  if (h->hf) return fail(h, VP_ERR_INVALID, "the HF front-end has no framing options");
   const bool kaldi = h->fe.kind == 0;
   const int m = o->frame_mode;
   if (kaldi ? (m != VP_FRAME_DEFAULT && m != VP_FRAME_KALDI_REFLECT)
@@ -213,6 +240,7 @@ int vp_frontend_set_options(vp_handle* h, const vp_frontend_options* o) {
 
 int32_t vp_num_frames(const vp_handle* h, int32_t n) {
   if (!h || !h->fe_set) return -1;
+  if (h->hf) return hf_frames(h->hf, n);
   return frontend_frames(h->fe.kind, h->fe_opt.frame_mode, h->fe.win_length, h->fe.n_fft, h->fe.hop, h->fe_opt.pad, n);
 }
 
@@ -230,6 +258,7 @@ static const char* frontend_length_error(const vp_handle* h, int L) {
 
 int32_t vp_feature_dim(const vp_handle* h) {
   if (!h || !h->fe_set) return -1;
+  if (h->hf) return hf_feature_dim(h->hf);
   return h->fe.post == 1 ? h->fe.n_out : h->fe.n_mels;
 }
 
@@ -244,6 +273,7 @@ static size_t frontend_scratch_floats(const vp_handle* h, int B, int T) {
   return n;
 }
 size_t vp_frontend_scratch_floats(const vp_handle* h, int32_t B, int32_t Lpad) {
+  if (h && h->fe_set && h->hf) return hf_scratch_floats(h->hf, B, Lpad);
   int T = vp_num_frames(h, Lpad);
   if (T <= 0) return 0;
   return frontend_scratch_floats(h, B, T) + round4((size_t)B);
@@ -252,6 +282,7 @@ size_t vp_frontend_scratch_floats(const vp_handle* h, int32_t B, int32_t Lpad) {
 // The waveform length check of every front-end call: "" when B rows of L samples give at least one frame.
 static const char* frontend_call_error(const vp_handle* h, int B, int L) {
   if (B < 1) return "empty batch";
+  if (h->hf) return hf_frames(h->hf, L) < 1 ? "shorter than the feature encoder's receptive field" : "";
   const char* len_err = frontend_length_error(h, L);
   if (*len_err) return len_err;
   return vp_num_frames(h, L) < 1 ? "shorter than one frame" : "";
@@ -285,6 +316,9 @@ static int run_frontend(vp_handle* h, const float* wave, int B, int L, const int
                         int T_call = -1) {
   if (!h) return VP_ERR_INVALID;
   if (!h->fe_set) return fail(h, VP_ERR_INVALID, "front-end not configured (vp_frontend_set)");
+  if (h->hf && B >= 1 && *frontend_call_error(h, B, L))     // a short row has no features to write: say why first
+    return fail(h, VP_ERR_INVALID, "waveform of %d samples: %s (%d samples): Kernel size can't be greater than actual "
+                "input size", L, frontend_call_error(h, B, L), hf_min_samples(h->hf));
   if ((stage != 2 && !wave) || (stage != 1 && !feats) || !scratch || B < 1) return fail(h, VP_ERR_INVALID, "null/empty argument");
   if (stage != 0 && (h->fe.post != 1 || !ext_max)) return fail(h, VP_ERR_INVALID, "two-stage calls are for the MFCC front-end");
   const char* len_err = frontend_call_error(h, B, L);
@@ -293,6 +327,11 @@ static int run_frontend(vp_handle* h, const float* wave, int B, int L, const int
     return fail(h, VP_ERR_INVALID, "T = %d frames: need 1 <= T <= %d, the frames of a %d-sample row", T_call,
                 vp_num_frames(h, L), L);
   CUDA_TRY(h, cudaSetDevice(h->device));
+  if (h->hf) {
+    if (stage != 0) return fail(h, VP_ERR_INVALID, "two-stage calls are for the MFCC front-end");
+    CUDA_TRY(h, hf_run(h->hf, wave, B, L, lens, lens ? T_call : vp_num_frames(h, L), keep, feats, scratch, st));
+    return VP_OK;
+  }
   FrontendParams p = frontend_params(h, B, L, lens ? T_call : -1);
   p.wave = wave; p.feats = feats; p.partial = scratch;
   const int T = p.T;
@@ -326,6 +365,10 @@ static int run_frontend(vp_handle* h, const float* wave, int B, int L, const int
 int vp_frontend_plan_info(const vp_handle* h, int32_t B, int32_t Lpad, int32_t stage, int32_t* info) {
   if (!h || !info) return VP_ERR_INVALID;
   if (!h->fe_set || stage != h->fe.post || *frontend_call_error(h, B, Lpad)) return VP_ERR_INVALID;
+  if (h->hf) {
+    hf_plan(h->hf, B, Lpad, info);
+    return VP_OK;
+  }
   const FrontendParams p = frontend_params(h, B, Lpad);
   const int inst = frontend_instantiation(p.N);
   info[0] = inst;
@@ -374,7 +417,7 @@ int vp_weights_load(vp_handle* h, const void* blob, size_t nbytes) {
 // ---------------------------------------------------------------------------------------------------------------
 // program validation: every offset/extent an op can touch is bounds-checked once here, so kernels run unchecked.
 // ---------------------------------------------------------------------------------------------------------------
-static bool act_ok(int a) { return a >= VP_ACT_NONE && a <= VP_ACT_SILU; }
+static bool act_ok(int a) { return a >= VP_ACT_NONE && a <= VP_ACT_GELU; }
 
 // extent (in floats) of a strided [rows, ld] view whose last row uses columns [coff, coff + cols)
 static size_t view_floats(long long rows, int ld, int coff, int cols) {

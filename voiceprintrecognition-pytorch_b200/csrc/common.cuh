@@ -81,6 +81,7 @@ __device__ __forceinline__ float apply_act(float v, int act) {
     case VP_ACT_SIGMOID: return 1.f / (1.f + expf(-v));
     case VP_ACT_TANH: return tanhf(v);
     case VP_ACT_SILU: return v / (1.f + expf(-v));
+    case VP_ACT_GELU: return 0.5f * v * (1.f + erff(v * 0.70710678118654752f));   // exact erf form
     default: return v;
   }
 }

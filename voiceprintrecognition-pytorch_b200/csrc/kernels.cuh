@@ -150,4 +150,21 @@ struct Res2Args {
 bool res2_chain_supported(int W, int T, int d);
 cudaError_t launch_res2_chain(Res2Args a, cudaStream_t stream);
 
+// Hugging Face wav2vec 2.0 / WavLM front-end (hf.cu): the handle owns one HfState (weights packed for the tensor-core
+// engine); frames, scratch and the launch sequence of a call come from here.
+struct HfState;
+const char* hf_desc_error(const vp_hf_desc& d);           // "" when the descriptor is one hf.cu runs
+cudaError_t hf_create(const vp_hf_desc& d, const float* const* conv_w, const float* const* conv_b,
+                      const float* const* norm_w, const float* const* norm_b, const float* proj_w, const float* proj_b,
+                      HfState** out);
+void hf_destroy(HfState* s);
+int hf_frames(const HfState* s, int64_t n);
+int hf_feature_dim(const HfState* s);
+int hf_min_samples(const HfState* s);                     // the shortest row with one output frame
+size_t hf_scratch_floats(const HfState* s, int B, int L);
+void hf_plan(const HfState* s, int B, int L, int32_t* info);
+// lens null: padded call (T = hf_frames(ld)); else ragged (T the longest row's frames).  keep: padded call only.
+cudaError_t hf_run(const HfState* s, const float* wave, int B, int ld, const int* lens, int T, const int* keep, float* feats,
+                   float* scratch, cudaStream_t st);
+
 }  // namespace vpb

@@ -10,7 +10,7 @@ ABI_VERSION = 5                 # VP_ABI_VERSION of include/vpb200.h
 VP_OK, VP_ERR_INVALID, VP_ERR_CUDA, VP_ERR_NOMEM, VP_ERR_UNSUPPORTED = 0, 1, 2, 3, 4
 OP_CONV, OP_CONV_C1, OP_COLSTATS, OP_ASP_POOL, OP_EW, OP_POOL2D = 1, 2, 3, 4, 5, 6
 POOL_MAX, POOL_AVG = 0, 1
-ACT_NONE, ACT_RELU, ACT_HARDTANH20, ACT_SIGMOID, ACT_TANH, ACT_SILU = 0, 1, 2, 3, 4, 5
+ACT_NONE, ACT_RELU, ACT_HARDTANH20, ACT_SIGMOID, ACT_TANH, ACT_SILU, ACT_GELU = 0, 1, 2, 3, 4, 5, 6
 PAD_ZERO, PAD_REFLECT = 0, 1
 SRC2_NONE, SRC2_ADD, SRC2_CONCAT = 0, 1, 2
 STATS_MEAN, STATS_MEAN_STD_CLAMP, STATS_MEAN_STD_UNBIASED, STATS_MEAN_STD_TSTP, STATS_SEG_CONTEXT = 0, 1, 2, 3, 4
@@ -33,6 +33,18 @@ FRAME_STFT_NOCENTER = 5
 
 class FrontendOptions(C.Structure):
     _fields_ = [('frame_mode', C.c_int32), ('pad', C.c_int32), ('spec_scale', C.c_double)]
+
+
+HF_MAX_LAYERS = 8
+HF_NORM_GROUP, HF_NORM_LAYER = 0, 1
+HF_SCRATCH_CAP = 1 << 28        # VP_HF_SCRATCH_CAP: floats of scratch one HF front-end slice may use
+
+
+class HfDesc(C.Structure):
+    _fields_ = [('n_layers', C.c_int32), ('conv_dim', C.c_int32 * HF_MAX_LAYERS),
+                ('conv_kernel', C.c_int32 * HF_MAX_LAYERS), ('conv_stride', C.c_int32 * HF_MAX_LAYERS),
+                ('conv_bias', C.c_int32), ('norm', C.c_int32), ('do_normalize', C.c_int32), ('norm_eps', C.c_float),
+                ('proj_eps', C.c_float)]
 
 
 class Op(C.Structure):
@@ -96,6 +108,8 @@ def lib():
         'vp_frontend_set': (C.c_int, [vp, C.POINTER(FrontendDesc), C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, i32, C.c_void_p]),
         'vp_frontend_set_options': (C.c_int, [vp, C.POINTER(FrontendOptions)]),
+        'vp_sizeof_hf_desc': (i32, []),
+        'vp_frontend_set_hf': (C.c_int, [vp, C.POINTER(HfDesc), pp, pp, pp, pp, C.c_void_p, C.c_void_p]),
         'vp_feature_dim': (i32, [vp]),
         'vp_num_frames': (i32, [vp, i32]),
         'vp_frontend_scratch_floats': (sz, [vp, i32, i32]),
@@ -148,8 +162,9 @@ def lib():
         raise RuntimeError('libvpb200.so ABI version mismatch')
     if L.vp_sizeof_op() != C.sizeof(Op) or L.vp_sizeof_frontend_desc() != C.sizeof(FrontendDesc) \
             or L.vp_sizeof_frontend_options() != C.sizeof(FrontendOptions) or L.vp_sizeof_flac_info() != C.sizeof(FlacInfo) \
-            or L.vp_sizeof_pcm_info() != C.sizeof(PcmInfo):
-        raise RuntimeError('vp_op / vp_frontend_desc / vp_frontend_options / vp_flac_info / vp_pcm_info layout mismatch '
+            or L.vp_sizeof_pcm_info() != C.sizeof(PcmInfo) or L.vp_sizeof_hf_desc() != C.sizeof(HfDesc):
+        raise RuntimeError('vp_op / vp_frontend_desc / vp_frontend_options / vp_flac_info / vp_pcm_info / vp_hf_desc '
+                           'layout mismatch '
                            'between the ctypes binding '
                            'and libvpb200.so')
     _lib = L
@@ -165,4 +180,5 @@ EXPORTS = ['vp_abi_version', 'vp_sizeof_op', 'vp_sizeof_frontend_desc', 'vp_crea
            'vp_spectral_scratch_bytes', 'vp_spectral_laplacian', 'vp_sym_tridiag', 'vp_sym_tridiag_apply_q',
            'vp_spectral_launches', 'vp_verify_scratch_bytes', 'vp_verify_metrics',
            'vp_resample', 'vp_gain_scratch_bytes', 'vp_gain_normalize', 'vp_frame_energy', 'vp_gather_windows',
-           'vp_sizeof_flac_info', 'vp_flac_scratch_bytes', 'vp_flac_decode', 'vp_sizeof_pcm_info', 'vp_pcm_decode']
+           'vp_sizeof_flac_info', 'vp_flac_scratch_bytes', 'vp_flac_decode', 'vp_sizeof_pcm_info', 'vp_pcm_decode',
+           'vp_sizeof_hf_desc', 'vp_frontend_set_hf']

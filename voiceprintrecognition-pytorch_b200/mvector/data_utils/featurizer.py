@@ -376,10 +376,33 @@ class MFCC:
                                        post=1, n_out=n_mfcc, db_mult=10.0, top_db=80.0)
 
 
+class HfFrontend:
+    """`use_hf_model`: the wav2vec 2.0 / WavLM checkpoint named by `feature_method` (a local directory or a hub id
+    already in the local cache, hf_checkpoint.resolve), lowered to the library's HF front-end (vp_frontend_set_hf):
+    processor normalisation, conv feature encoder, feature projection LayerNorm -- everything `extract_features`
+    depends on (featurizer.py:65-73).  `method_args['use_gpu']` is accepted and ignored, as on the reference's GPU."""
+
+    def __init__(self, name, method_args):
+        from .hf_checkpoint import HfCheckpoint
+        self.ckpt = HfCheckpoint(name)
+        c = self.ckpt
+        n = len(c.conv_dim)
+        if n > L.HF_MAX_LAYERS:
+            raise NotImplementedError(f'{n} conv layers: the HF front-end runs at most {L.HF_MAX_LAYERS}')
+        pad = lambda v: (C.c_int32 * L.HF_MAX_LAYERS)(*(list(v) + [0] * (L.HF_MAX_LAYERS - n)))
+        self.hf_desc = L.HfDesc(n_layers=n, conv_dim=pad(c.conv_dim), conv_kernel=pad(c.conv_kernel),
+                                conv_stride=pad(c.conv_stride), conv_bias=int(c.conv_bias),
+                                norm=L.HF_NORM_GROUP if c.norm == 'group' else L.HF_NORM_LAYER,
+                                do_normalize=int(c.do_normalize), norm_eps=1e-5, proj_eps=c.layer_norm_eps)
+        self.n_mels = max(c.conv_dim)
+        self.desc = L.FrontendDesc(kind=2, post=0, top_db=-1.0)     # what the featurizer asks of every front-end
+
+
 class AudioFeaturizer:
     """音频特征器 (drop-in for mvector.data_utils.featurizer.AudioFeaturizer).
 
-    :param feature_method: 'Fbank' | 'MelSpectrogram' | 'Spectrogram' | 'MFCC'  (HF models: not lowered, raise)
+    :param feature_method: 'Fbank' | 'MelSpectrogram' | 'Spectrogram' | 'MFCC', or with use_hf_model a wav2vec 2.0 /
+        WavLM checkpoint (local directory or cached hub id, HfFrontend)
     :param method_args: forwarded as **kwargs exactly like the reference (unknown keys -> TypeError)
     """
 
@@ -388,8 +411,8 @@ class AudioFeaturizer:
         self._feature_method = feature_method
         self.use_hf_model = use_hf_model
         if use_hf_model:
-            raise NotImplementedError('HF wav2vec-style feature models are outside the lowered path (SURVEY.md 2)')
-        if feature_method == 'MelSpectrogram':
+            self.feat_fun = HfFrontend(feature_method, method_args)
+        elif feature_method == 'MelSpectrogram':
             self.feat_fun = MelSpectrogram(**method_args)
         elif feature_method == 'Fbank':
             self.feat_fun = KaldiFbank(**method_args)
@@ -402,7 +425,10 @@ class AudioFeaturizer:
         self.whole_call = self.feat_fun.desc.post == 1 and self.feat_fun.desc.top_db >= 0    # MFCC's call-wide clamp
         self._engine = engine
         self._configured = False
-        logger.info(f'使用【{feature_method}】提取特征')
+        if use_hf_model:
+            logger.info(f'使用模型【{feature_method}】提取特征，使用【cuda】设备提取')
+        else:
+            logger.info(f'使用【{feature_method}】提取特征')
 
     # -- lazy device state so that constructing the object (config parsing) needs no GPU --
     def _ensure(self):
@@ -411,6 +437,10 @@ class AudioFeaturizer:
         if self._engine is None:
             self._engine = Engine()
         f = self.feat_fun
+        if self.use_hf_model:
+            self._set_hf(f)
+            self._configured = True
+            return
         start, count, off, w = f.bank
         win = np.ascontiguousarray(f.window, dtype=np.float32)
         dct = getattr(f, 'dct', None)
@@ -421,6 +451,30 @@ class AudioFeaturizer:
         _check(self._engine.handle, L.lib().vp_frontend_set_options(self._engine.handle, C.byref(f.opts)))
         self._configured = True
 
+    def _set_hf(self, f):
+        c = f.ckpt
+        n, wt = len(c.conv_dim), c.weights
+        keep = []                                        # the host arrays stay alive until the library has copied them
+
+        def ptrs(names):
+            arr = (C.c_void_p * L.HF_MAX_LAYERS)()
+            for i, k in enumerate(names):
+                if k in wt:
+                    a = np.ascontiguousarray(wt[k], dtype=np.float32)
+                    keep.append(a)
+                    arr[i] = a.ctypes.data
+            return arr
+        cw = ptrs([f'feature_extractor.conv_layers.{i}.conv.weight' for i in range(n)])
+        cb = ptrs([f'feature_extractor.conv_layers.{i}.conv.bias' for i in range(n)])
+        nw = ptrs([f'feature_extractor.conv_layers.{i}.layer_norm.weight' for i in range(n)])
+        nb = ptrs([f'feature_extractor.conv_layers.{i}.layer_norm.bias' for i in range(n)])
+        pw = np.ascontiguousarray(wt['feature_projection.layer_norm.weight'], dtype=np.float32)
+        pb = np.ascontiguousarray(wt['feature_projection.layer_norm.bias'], dtype=np.float32)
+        pp = C.POINTER(C.c_void_p)
+        _check(self._engine.handle, L.lib().vp_frontend_set_hf(
+            self._engine.handle, C.byref(f.hf_desc), C.cast(cw, pp), C.cast(cb, pp), C.cast(nw, pp), C.cast(nb, pp),
+            pw.ctypes.data_as(C.c_void_p), pb.ctypes.data_as(C.c_void_p)))
+
     @property
     def engine(self):
         self._ensure()
@@ -430,6 +484,8 @@ class AudioFeaturizer:
         """Frames T for a waveform of n_samples (vp_num_frames): kaldi._get_strided, or torch.stft of the `pad`-extended
         signal, centred or not."""
         f = self.feat_fun
+        if self.use_hf_model:
+            return f.ckpt.num_frames(n_samples)
         mode = f.opts.frame_mode
         if f.desc.kind == 0:
             if mode == L.FRAME_KALDI_REFLECT:
@@ -548,7 +604,9 @@ class AudioFeaturizer:
 
     @property
     def feature_dim(self):
-        """featurizer.py:93-111."""
+        """featurizer.py:93-111 (the HF model's output channels: conv_dim[-1])."""
+        if self.use_hf_model:
+            return self.feat_fun.ckpt.feature_dim
         if self._feature_method == 'MelSpectrogram':
             return self._method_args.get('n_mels', 128)
         elif self._feature_method == 'Spectrogram':
